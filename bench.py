@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """bench.py — images/sec of one training iteration of TestModel (ResNet-50 encoder, 320×320, bs 16/GPU, bf16)
-through the B200 hot path, with the CPU reference timed beside it.
+through the H100 hot path, with the CPU reference timed beside it.
 
     python bench.py [--gpus N --steps K --warmup W]                      # this repo's arm
     python -m torch.distributed.run --nproc-per-node N ... bench.py --gpus N ...
@@ -11,7 +11,8 @@ One JSON line on stdout (rank 0).  `value` = whole-job images/s with the batch a
 `e2e` = the same through `Trainer.step_from_host` (pinned host batch → H2D → iteration → loss D2H);
 `roofline` = the dominant hand-written kernel (SyncBN backward) replayed on the model's 84 layer shapes and
 timed with CUDA events on the launching stream; `cpu_baseline` = the oracle restatement of the reference loop
-on the host cores (bounded sample).  Nothing here reads /root/reference.
+on the host cores (bounded sample).  Nothing here reads the reference project.
+`--dump-outputs DIR` writes what the timed path returned in its last timed step as DIR/<name>.npy.
 """
 from __future__ import annotations
 
@@ -50,14 +51,48 @@ def parse():
                     help="BASELINE config 4: one size of {256,320,384} per batch (rank-shared RNG), as the reference's multi-scale collate")
     ap.add_argument("--no-parity-check", action="store_true", help="skip the untimed world>1 parity leg")
     ap.add_argument("--no-extras", action="store_true", help="skip the ride-along measurements (multi-scale, sweep, stock-torch arm)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="GPU arms: write the loss, per-pixel logits and a fixed sample of the updated parameters of the last "
+                         "timed step as DIR/<name>.npy (float32), so that two builds can be compared output for output; "
+                         "cuDNN then runs deterministically (no autotuning), so the timing is not the headline configuration")
     return ap.parse_args()
 
 
+NVLINK_GBS = 450.0      # H100 SXM, NVLink 4: 18 links, 450 GB/s per direction per GPU (data sheet)
+
+
 def peaks():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        return json.load(open(p)), "measured"
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0}, "fallback"
+    """H100 SXM data sheet (700 W card): HBM3 bandwidth and dense BF16 rate.  A fraction of these is a share of the data
+    sheet, not of what the card at hand reaches; `gpu` in the JSON line names the card and its power limit."""
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0}, "datasheet"
+
+
+def gpu_info(index: int) -> dict:
+    """name, power limit and maximum SM clock of the GPU the numbers were measured on"""
+    info = {"name": torch.cuda.get_device_name(index)}
+    try:
+        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader,nounits",
+                              "-i", str(index)], capture_output=True, text=True, timeout=30).stdout.strip().split(",")
+        if len(out) == 3:
+            info.update(power_limit_w=float(out[1]), sm_max_mhz=float(out[2]))
+    except (OSError, ValueError, subprocess.SubprocessError):
+        pass
+    return info
+
+
+def dump_outputs(path: str, out, params) -> None:
+    """`out` = (loss, loss items, logits) as the timed step returned them; `params` = the model's parameters after that
+    step, of which a fixed seeded sample of 2^20 values is kept (the full set is 100 MB)."""
+    import numpy as np
+    os.makedirs(path, exist_ok=True)
+    loss, items, preds = out
+    flat = torch.cat([p.detach().reshape(-1).float() for p in params])
+    idx = torch.randperm(flat.numel(), generator=torch.Generator().manual_seed(0))[:1 << 20].sort().values
+    arrays = {"loss": loss, "logits": preds, "params_sample": flat[idx.to(flat.device)]}
+    if torch.is_tensor(items):
+        arrays["loss_items"] = items
+    for name, t in arrays.items():
+        np.save(os.path.join(path, f"{name}.npy"), t.detach().float().cpu().numpy())
 
 
 class ClockSampler:
@@ -285,7 +320,7 @@ def bn_roofline(trace, dtype, iters=5):
         e.synchronize()
         return s.elapsed_time(e)
 
-    # Every launch starts cold: a 256 MB write flushes the 126 MB L2 before it, INSIDE the event pair, and the flush's own
+    # Every launch starts cold: a 256 MB write flushes the 50 MB L2 before it, INSIDE the event pair, and the flush's own
     # time (measured the same way, median) is subtracted.  A pair of events around one 15 µs kernel would mostly measure the
     # events themselves (≈4 µs); here the kernel's launch overlaps the preceding flush, as it overlaps the preceding
     # convolution in the real iteration.
@@ -591,7 +626,7 @@ def extra_sweep(world, timed):
             iters = 20 if nbytes <= (16 << 20) else 8
             us = timed(lambda i: fn(), iters) / iters * 1e3
             row[name] = {"us": us, "bus_gbs": 2 * (world - 1) / world * nbytes / (us * 1e-6) / 1e9}
-        row["frac_of_nvlink_900"] = row["sod"]["bus_gbs"] / 900.0
+        row["frac_of_nvlink"] = row["sod"]["bus_gbs"] / NVLINK_GBS
         rows.append(row)
     arena.check_error()
     return {"world": world, "multicast": arena.has_multicast, "rows": rows}
@@ -657,7 +692,10 @@ def run_b200_arm(args):
 
     dtype = torch.bfloat16 if args.dtype == "bf16" else torch.float32
     args.warmup = max(3, args.warmup)          # timing rule: at least 3 warm-up iterations
-    torch.backends.cudnn.benchmark = True
+    # a dump has to be reproducible: cuDNN's timed algorithm choice and its non-deterministic kernels would make two runs
+    # of one build differ after a few training steps, so --dump-outputs runs cuDNN deterministically (and slower)
+    torch.backends.cudnn.benchmark = not args.dump_outputs
+    torch.backends.cudnn.deterministic = bool(args.dump_outputs)
     if os.environ.get("SOD_CUDNN_BENCH_LIMIT"):      # experiment knob: 0 = let cuDNN's autotuner try every engine (default 10)
         torch.backends.cudnn.benchmark_limit = int(os.environ["SOD_CUDNN_BENCH_LIMIT"])
     log('building trainer')
@@ -684,7 +722,7 @@ def run_b200_arm(args):
         mean_pixels = sum(sizes[k] ** 2 for k in order[:args.warmup + args.steps][args.warmup:]) / max(args.steps, 1)
     else:
         host = [synth_batch(1234 + rank + 100 * i, BS, SIZE) for i in range(nb)]
-        pick = [i % nb for i in range(8192)]
+        pick = [i % nb for i in range(nb)]
         mean_pixels = SIZE * SIZE
     host = [(x.pin_memory(), m.pin_memory()) for x, m in host]
     dev = [(x.cuda(non_blocking=True), m.cuda(non_blocking=True)) for x, m in host]
@@ -715,7 +753,7 @@ def run_b200_arm(args):
     for i in range(args.warmup):
         if i == trace_at:
             syncbn.TRACE = []
-        tr.forward_backward_update(*dev[pick[i]])
+        tr.forward_backward_update(*dev[pick[i % len(pick)]])
         torch.cuda.synchronize(); log(f'warmup {i} done')
         if i == trace_at:
             trace, syncbn.TRACE = syncbn.TRACE, None
@@ -731,19 +769,26 @@ def run_b200_arm(args):
     rid = torch.cuda.nvtx.range_start("timed")      # start/end range: process-wide (backward runs on autograd's thread)
     clk.mark()
     w0 = args.warmup
-    ms = timed(lambda i: tr.forward_backward_update(*dev[pick[w0 + i]]), args.steps)
+    last = {}
+
+    def timed_step(i):
+        last["out"] = tr.forward_backward_update(*dev[pick[(w0 + i) % len(pick)]])
+    ms = timed(timed_step, args.steps)
     clk.mark()
     torch.cuda.nvtx.range_end(rid)
     clk.__exit__()
     launches = _lib.launches - l0
     log(f'timed region done: {ms / args.steps:.2f} ms/step')
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last["out"], tr.module.parameters())
     value = world * BS * args.steps / (ms * 1e-3)
 
     # -- end-to-end arm: pinned host batch in, loss out, every step ------------------------------------
     for i in range(min(args.warmup, 3)):
         tr.step_from_host(*host[pick[i]])
     tr.last_loss()
-    ms_e2e = timed(lambda i: (tr.step_from_host(*host[pick[w0 + i]]), tr.last_loss() if i == args.steps - 1 else None), args.steps)
+    ms_e2e = timed(lambda i: (tr.step_from_host(*host[pick[(w0 + i) % len(pick)]]), tr.last_loss() if i == args.steps - 1 else None),
+                   args.steps)
     e2e = world * BS * args.steps / (ms_e2e * 1e-3)
     log(f'e2e done: {ms_e2e / args.steps:.2f} ms/step')
     if args.impl == "torch":
@@ -788,7 +833,7 @@ def run_b200_arm(args):
         if world > 1:
             bus = 2.0 * (world - 1) / world * 4.0 * flat.numel / (us_step * 1e-6) / 1e9
             extras["fused_allreduce_sgd"] = {"us": us_step, "flat_elems": flat.numel, "params": n_real, "bus_gbs": bus,
-                                             "frac_of_nvlink_900": bus / 900.0,
+                                             "frac_of_nvlink": bus / NVLINK_GBS,
                                              "note": "multi-tensor gather + [reduce-scatter(grad, bf16 on the wire) + SGD + all-gather(param)] in one kernel"}
         else:
             per = 22 if flat.grad16 is not None else 24   # bf16 gradient in (2) + p, v in/out (16) + bf16 shadow out (2) + clear (2) | g, p, v + clear
@@ -830,12 +875,6 @@ def run_b200_arm(args):
             "achieved": bw, "peak": pk["hbm_gbs"], "unit": "GB/s", "frac": bw / pk["hbm_gbs"], "peak_kind": pk_kind,
             "how": "84 launches of one iteration replayed; per layer: CUDA events around 4 x [256 MB L2 flush + launch], flush time subtracted",
             "traffic": None, "avg_launch_ms": avg_ms, "algorithmic_bytes_per_launch": avg_bytes}
-    try:        # dram__bytes_read + dram__bytes_write per launch, from the committed ncu pass over the same 84 launches (tools/bn_dram.py)
-        dram = json.load(open(os.path.join(ROOT, "profiles", "r02_syncbn_bwd_dram.json")))
-        roof["traffic"] = dram["avg_dram_bytes_per_launch"]
-        roof["traffic_source"] = "profiles/r02_syncbn_bwd_dram.json (ncu dram__bytes_read.sum + dram__bytes_write.sum, each launch cold)"
-    except (OSError, KeyError, ValueError):
-        roof["traffic_source"] = "no committed ncu capture for this kernel revision"
     line = {"metric": METRIC, "value": value, "unit": UNIT, "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
             "ms_per_step": ms / args.steps, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
             "dtype": args.dtype, "data": "synthetic",
@@ -846,8 +885,8 @@ def run_b200_arm(args):
                                    "fwd (cuDNN convs NHWC + fused SyncBN kernels) + fused BCE/CEL fwd+bwd + bwd + "
                                    "fused (all-reduce+)SGD-momentum", "global_batch": BS * world,
                        "parallelism": f"dp{world}", "l2": "4 rotating input batches; per-iteration working set (>5 GB of "
-                                                          "activations) far exceeds the 126 MB L2, no explicit flush"},
-            "clocks": clk.summary(),
+                                                          "activations) far exceeds the 50 MB L2, no explicit flush"},
+            "clocks": clk.summary(), "gpu": gpu_info(local),
             "e2e": {"value": e2e, "unit": UNIT, "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": 4, "ms_per_step": ms_e2e / args.steps},
             "gpu_launches": launches, "roofline": roof}
     try:        # the loss kernel alone: at the workload shape (latency bound) and at SURVEY §8d's scaled shape
@@ -928,7 +967,7 @@ def run_sweep(args):
         rows.append(res)
     arena.check_error()
     if rank == 0:
-        print(json.dumps({"sweep": "allreduce", "world": world, "multicast": arena.has_multicast, "nvlink_peak_gbs": 900,
+        print(json.dumps({"sweep": "allreduce", "world": world, "multicast": arena.has_multicast, "nvlink_peak_gbs": NVLINK_GBS,
                           "rows": rows}), flush=True)
     dist.barrier(); dist.destroy_process_group()
 

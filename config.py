@@ -1,12 +1,12 @@
 """Experiment configuration — same keys and semantics as the reference's `config.py:25-76`.
 
-Two DEFAULTS differ from the reference on purpose: `use_amp` is True (the reference ships False; bf16 autocast is the B200
-configuration BASELINE names) and `resume_mode` is "" (the reference ships "test", which evaluates an existing checkpoint and
+Two DEFAULTS differ from the reference on purpose: `use_amp` is True (the reference ships False; bf16 autocast is the benchmark
+configuration) and `resume_mode` is "" (the reference ships "test", which evaluates an existing checkpoint and
 exits — a fresh checkout has none).  Every other default is the reference's.
 
-Extra keys (all optional, defaults reproduce the B200 benchmark configuration):
+Extra keys (all optional, defaults reproduce the benchmark configuration):
   dtype           "bf16" | "fp16" | "fp32": autocast dtype used when `use_amp` is True
-  channels_last   run the network in NHWC (what cuDNN's Blackwell kernels and the SyncBN kernels want)
+  channels_last   run the network in NHWC (what cuDNN's tensor-core kernels and the SyncBN kernels want)
   synthetic       train on synthetic batches of the dataloader's output contract (no dataset on this machine)
   cuda_graph      capture one iteration per (shape, lr) and replay it: one launch instead of ~700 kernel launches
 """
@@ -64,7 +64,7 @@ user_config = {
     "num_workers": 4,
     "input_size": 320,
     "proj_root": proj_root,
-    # --- B200 engine extras ---
+    # --- engine extras ---
     "dtype": "bf16",
     "channels_last": True,
     "synthetic": True,

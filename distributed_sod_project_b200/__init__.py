@@ -1,2 +1,2 @@
-"""B200-native data-parallel hot path for lartpang/Distributed-SOD-Project (see DESIGN.md)."""
+"""H100-native data-parallel hot path for lartpang/Distributed-SOD-Project (see DESIGN.md)."""
 __version__ = "0.1.0"

@@ -1,7 +1,7 @@
 """amp seam: `amp.initialize`, `amp.scale_loss`, `amp.state_dict/load_state_dict` of the reference
 (apex.amp O1; train.py:15,181-183,298-300, utils/pipeline_ops.py:74,121).
 
-B200 default: bf16 autocast, loss scale fixed at 1.0 — bf16 has fp32's exponent range, so the dynamic
+Default: bf16 autocast, loss scale fixed at 1.0 — bf16 has fp32's exponent range, so the dynamic
 scaler of apex O1 has nothing to do; weights, gradients and optimizer state stay fp32 ("fp32 master") exactly
 as under O1.  `dtype=torch.float16` keeps apex's dynamic-scale behaviour (init 2^16, ÷2 and skip the step on
 overflow, ×2 every 2000 clean steps): the unscale factor and the overflow flag are consumed INSIDE the fused

@@ -17,6 +17,7 @@ const DevInfo& dev_info() {
         cudaDeviceGetAttribute(&d.cc_major, cudaDevAttrComputeCapabilityMajor, dev);
         cudaDeviceGetAttribute(&d.cc_minor, cudaDevAttrComputeCapabilityMinor, dev);
         cudaDeviceGetAttribute(&d.max_smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
+        cudaDeviceGetAttribute(&d.l2_bytes, cudaDevAttrL2CacheSize, dev);
     }
     return d;
 }
@@ -31,7 +32,7 @@ extern "C" const char* sod_strerror(int code) {
         case SOD_EINVAL: return "invalid argument (null pointer, non-positive size or bad enum)";
         case SOD_EALIGN: return "pointer or offset is not 16-byte aligned";
         case SOD_EWORKSPACE: return "workspace too small";
-        case SOD_EUNSUPPORTED: return "unsupported shape / dtype combination or not an sm_100 device";
+        case SOD_EUNSUPPORTED: return "unsupported shape / dtype combination or not an sm_90 device";
         case SOD_ECOMM: return "invalid communicator";
         default: break;
     }

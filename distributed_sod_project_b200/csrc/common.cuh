@@ -1,4 +1,4 @@
-// common.cuh — device helpers shared by the sm_100a kernels of libsod_b200.so.
+// common.cuh — device helpers shared by the sm_90a kernels of libsod_b200.so.
 #pragma once
 #include <cooperative_groups.h>
 #include <cuda_bf16.h>
@@ -23,7 +23,7 @@ static inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t
 // device properties (cached per device)
 // ------------------------------------------------------------------------------------------------
 struct DevInfo {
-    int sm_count = 0, cc_major = 0, cc_minor = 0, max_smem_optin = 0;
+    int sm_count = 0, cc_major = 0, cc_minor = 0, max_smem_optin = 0, l2_bytes = 0;
 };
 const DevInfo& dev_info();  // api.cu
 

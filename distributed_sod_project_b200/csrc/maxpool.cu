@@ -4,9 +4,8 @@
 // EXPERIMENTAL: written after round 1's GPU budget was spent — compiled and exported, but the host layer keeps it off
 // (resample.MAXPOOL_ENABLED) until it has been checked against torch on hardware.
 //
-// Why: on [16,64,160,160] bf16 torch's `max_pool_forward_nhwc` + `max_pool_backward_nhwc` take 148 + 247 µs per iteration
-// (profiles/r01_ncu_launches.csv) for ≈75 MB of compulsory traffic each (≈15 µs at HBM speed); the backward drags an
-// int64 index tensor (4× the size of the bf16 output).  Here: 16-byte channel packets, one byte of window position
+// Why: on [16,64,160,160] bf16 torch's `max_pool_forward_nhwc` + `max_pool_backward_nhwc` move ≈75 MB of compulsory
+// traffic each, and the backward drags an int64 index tensor (4× the size of the bf16 output).  Here: 16-byte channel packets, one byte of window position
 // (kh*3+kw) per element instead of an int64 flat index, and a gather backward (every input pixel looks at the ≤4 windows
 // that contain it, in ascending window order) — deterministic, fp32 accumulation like torch's.
 // Tie-breaking and NaN behaviour follow torch's kernels: scan kh, kw ascending, replace on (v > max || isnan(v)),

@@ -499,8 +499,8 @@ extern "C" int sod_allreduce_sgd(const sod_comm* comm, uint64_t grad_off, uint64
     const unsigned grid = comm_grid((nvec + c.world - 1) / c.world);
     const float scale = inv_scale / static_cast<float>(c.world);
     const int zg = (flags & SOD_SGD_ZERO_GRAD) ? 1 : 0;
-    // measured (profiles/r01_allreduce_sweep_w2.json): with two ranks the in-switch reduction loses to plain peer loads
-    // (288 vs 175 µs at 99.6 MB); from four ranks up NVLS wins (281 vs 346 µs at eight)
+    // with two ranks plain peer loads move the gradient bucket faster than the in-switch reduction; from four ranks up
+    // NVLS wins (an all-reduce sweep, `bench.py --sweep`, decides this per system)
     const bool mc = (c.mc != 0) && !(flags & SOD_ALGO_NO_MULTIMEM) && (c.world > 2 || (flags & SOD_ALGO_FORCE_MULTIMEM));
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     if (mc)
@@ -525,9 +525,8 @@ extern "C" int sod_allreduce_f32(const sod_comm* comm, uint64_t off, int64_t n, 
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     const long long one_shot_cap = static_cast<long long>(kThreads) * kUnroll *
                                    (dev_info().sm_count < SOD_COMM_MAX_BLOCKS ? dev_info().sm_count : SOD_COMM_MAX_BLOCKS);
-    // measured (profiles/r02_call3_w2_sweep_w2.txt, extras.allreduce_sweep of the 4/8-GPU lines): the two-shot kernel over the
-    // NVLS mapping beats the one-shot kernel at every size once a multicast mapping exists (64 KB: 17-20 µs vs 24-43 µs);
-    // one-shot (every rank reads every peer) is only kept for fabrics without multicast
+    // the two-shot kernel over the NVLS mapping beats the one-shot kernel at every size once a multicast mapping exists
+    // (`bench.py --sweep`); one-shot (every rank reads every peer) is only kept for fabrics without multicast
     const bool has_mc = (c.mc != 0) && !(flags & SOD_ALGO_NO_MULTIMEM);
     if (algo == 0) algo = (!has_mc && n * 4 <= (256 << 10)) ? 1 : 2;
     if (algo == 1 && nvec > one_shot_cap) return SOD_EUNSUPPORTED;
@@ -536,7 +535,7 @@ extern "C" int sod_allreduce_f32(const sod_comm* comm, uint64_t off, int64_t n, 
         allreduce_one_shot_kernel<<<grid, kThreads, 0, s>>>(c, off, nvec, scale);
     } else {
         const unsigned grid = comm_grid((nvec + c.world - 1) / c.world);
-        // in-switch reduction: always from four ranks up; with two ranks peer loads win above ≈2 MB (99.6 MB: 176 vs 288 µs)
+        // in-switch reduction: always from four ranks up; with two ranks peer loads win above ≈2 MB
         const bool mc = has_mc && (c.world > 2 || n * 4 <= (2 << 20) || (flags & SOD_ALGO_FORCE_MULTIMEM));
         if (mc) allreduce_two_shot_kernel<true><<<grid, kThreads, 0, s>>>(c, off, nvec, scale);
         else allreduce_two_shot_kernel<false><<<grid, kThreads, 0, s>>>(c, off, nvec, scale);

@@ -13,7 +13,7 @@
 //   stage   the strip is pulled through a ring of shared-memory stages (32-48 KB each) by 1-D bulk async
 //           copies (TMA engine, mbarrier completion) issued by a dedicated producer warp: ≈150 KB per
 //           SM in flight with no registers tied up (geometry from tools/membench.cu: a bulk-copy ring
-//           delivers ∝ bytes per stage; 32 KB reaches ≈7 TB/s, 8 KB only 3);
+//           delivers ∝ bytes per stage, so stages are 32-48 KB rather than 8);
 //   fold    biases of the convolutions that produced x / pre_add are added here (z = x + pre + b),
 //           and their gradient Σ dz comes out of the backward's own statistics;
 //   phase 1 per-thread fp32 partial sums straight from shared memory → CTA total [2C];
@@ -1099,9 +1099,8 @@ __global__ void __launch_bounds__(kBlock, 1) syncbn_bwd_kernel(const __grid_cons
 
 // ---- host side ------------------------------------------------------------------------------------------
 static int make_geom(int64_t rows, int C, int dtype, int nstream, BnGeom& g, int max_chunk = 32768) {
-    // tools/membench.cu: a bulk-copy ring delivers ∝ bytes per chunk iteration (fixed ≈0.4 µs per iteration):
-    // 32-48 KB per stage reaches ≈7 TB/s, 16 KB only 5.5, 8 KB 3.1.  So: the largest power-of-two chunk per stream
-    // with nstream*chunk <= 48 KB.
+    // tools/membench.cu: a bulk-copy ring delivers ∝ bytes per chunk iteration (a fixed cost per iteration), so
+    // small stages leave bandwidth unused.  So: the largest power-of-two chunk per stream with nstream*chunk <= 48 KB.
     int chunk_bytes = max_chunk;
     while (nstream * chunk_bytes > 49152) chunk_bytes >>= 1;
     if (rows <= 0 || C <= 0 || (C % 8) != 0 || C > kMaxC) return SOD_EUNSUPPORTED;
@@ -1127,7 +1126,7 @@ static int make_geom(int64_t rows, int C, int dtype, int nstream, BnGeom& g, int
     long long cap = dv.sm_count < kMaxGrid ? dv.sm_count : kMaxGrid;
     // hop-1 packets cost strips*2C*8 bytes of traffic: keep that well below the tensor itself
     const long long tensor_bytes = rows * C * g.es;
-    static const long long traffic_div = [] {          // experiment knob (tools/r2_call17.sh): SOD_BN_TRAFFIC_DIV, default 4
+    static const long long traffic_div = [] {          // experiment knob: SOD_BN_TRAFFIC_DIV, default 4
         const char* e = getenv("SOD_BN_TRAFFIC_DIV");
         const long long v = e ? atoll(e) : 4;
         return v >= 1 ? v : 4;
@@ -1227,7 +1226,7 @@ extern "C" int sod_syncbn_fwd(const void* x, const void* pre_add, const void* re
     SOD_CHECK_ARG((running_mean == nullptr) == (running_var == nullptr), SOD_EINVAL);
     SOD_CHECK_ARG(aligned16(x) && aligned16(y) && aligned16(workspace) && (!pre_add || aligned16(pre_add)) &&
                       (!residual || aligned16(residual)), SOD_EALIGN);
-    if (dev_info().cc_major != 10) return SOD_EUNSUPPORTED;
+    if (dev_info().cc_major != 9) return SOD_EUNSUPPORTED;
     BnFwd p{};
     int rc = make_comm_dev(training ? comm : nullptr, p.c);
     if (rc != SOD_OK) return rc;
@@ -1278,7 +1277,7 @@ extern "C" int sod_syncbn_bwd(const void* dy, const void* x, const void* pre_add
     SOD_CHECK_ARG(!relu || y || xmask, SOD_EINVAL);
     SOD_CHECK_ARG(aligned16(dy) && aligned16(x) && aligned16(dz) && aligned16(workspace) &&
                       (!pre_add || aligned16(pre_add)) && (!y || aligned16(y)) && (!dres || aligned16(dres)), SOD_EALIGN);
-    if (dev_info().cc_major != 10) return SOD_EUNSUPPORTED;
+    if (dev_info().cc_major != 9) return SOD_EUNSUPPORTED;
     BnBwd p{};
     int rc = make_comm_dev(comm, p.c);
     if (rc != SOD_OK) return rc;
@@ -1296,7 +1295,7 @@ extern "C" int sod_syncbn_bwd(const void* dy, const void* x, const void* pre_add
     {   // HINT: a layer whose operands cannot all sit in L2 anyway writes its outputs evict-first, so that the part of the
         // strip phase 2 still has to fetch is not pushed out by them; a small layer keeps its outputs for the consumer
         const long long footprint = static_cast<long long>(rows) * channels * (dtype == SOD_F32 ? 4 : 2) * (nstream + 1 + (dres ? 1 : 0));
-        p.store_policy = footprint > (96ll << 20) ? kL2EvictFirst : kL2EvictNormal;
+        p.store_policy = footprint > static_cast<long long>(dev_info().l2_bytes) * 3 / 4 ? kL2EvictFirst : kL2EvictNormal;
     }
     p.gamma = gamma; p.smean = save_mean; p.sinvstd = save_invstd; p.dgamma = dgamma; p.dbeta = dbeta;
     p.relu = relu; p.stats_off = stats_off; p.tag = seq; p.epoch = epoch;

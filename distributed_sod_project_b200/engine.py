@@ -1,4 +1,4 @@
-"""One training iteration of the reference (train.py:284-310), wired onto the B200 kernels.
+"""One training iteration of the reference (train.py:284-310), wired onto the sm_90a kernels.
 
 `Trainer` performs exactly the construction sequence of the reference's `main_worker` (train.py:141-207):
 model factory → make_optimizer → convert_syncbn_model → amp.initialize → DDP → loss list; and `step` is the
@@ -18,8 +18,8 @@ from .parallel import DistributedDataParallel
 from .syncbn import convert_syncbn_model
 from .utils import init_seed
 
-# overlap the next batch's host→device copy with the running iteration (see Trainer._stage_inputs); validated on B200 in
-# round 2 (profiles/r02_call1_*): e2e 1444 → 1559 img/s.  SOD_E2E_PREFETCH=0 restores the serialized copy.
+# overlap the next batch's host→device copy with the running iteration (see Trainer._stage_inputs).
+# SOD_E2E_PREFETCH=0 restores the serialized copy.
 PREFETCH_H2D = os.environ.get("SOD_E2E_PREFETCH", "1") == "1"
 
 
@@ -30,7 +30,7 @@ class Trainer:
                  device: torch.device | None = None, report_items: bool = True, use_graph: bool = False,
                  native_interpolate: bool = True, shadow_weights: bool = True):
         if not torch.cuda.is_available():
-            raise RuntimeError("the B200 engine needs a CUDA device")
+            raise RuntimeError("the engine needs a CUDA device")
         self.device = device or torch.device("cuda", torch.cuda.current_device())
         self.world = comm.world_size()
         self.channels_last = channels_last

@@ -1,4 +1,4 @@
-"""Loss seam of the reference, backed by the fused sm_100a kernel (csrc/loss.cu).
+"""Loss seam of the reference, backed by the fused sm_90a kernel (csrc/loss.cu).
 
 Reference surface kept (paths in the reference repo):
 * `BCEWithLogitsLoss(reduction=...)`  — train.py:203

@@ -1,7 +1,7 @@
 """Building blocks of the TestModel plugin family (`res50`, `cp_res50`).
 
 Written from scratch for this repo; the *contract* it keeps is the reference's
-(`/root/reference`):
+(lartpang/Distributed-SOD-Project):
 
 * parameter / buffer names and registration order of `network/TestModel.py:17-185`,
   `module/BaseBlocks.py:10-40`, `module/MyLightModule.py:11-54`,
@@ -10,11 +10,11 @@ Written from scratch for this repo; the *contract* it keeps is the reference's
   `div_2` / `div*` prefixes, `utils/pipeline_ops.py:295-303`);
 * RNG consumption order at construction, so that `init_seed(0)` followed by the factory call
   yields bit-identical initial weights to the reference (checked by
-  tests/test_host_cpu.py::test_model_plugin_is_bit_identical_to_reference when /root/reference is present).
+  tests/test_host_cpu.py::test_model_plugin_is_bit_identical_to_reference against vectors of the reference's model).
 
-Every BatchNorm site goes through :func:`bn_act`, which is where the B200 engine hooks in:
+Every BatchNorm site goes through :func:`bn_act`, which is where the engine hooks in:
 after `convert_syncbn_model` the BN modules expose `fused_forward`, and the (pre-add → BN →
-residual-add → ReLU) chain becomes one hand-written sm_100a kernel instead of up to four
+residual-add → ReLU) chain becomes one hand-written sm_90a kernel instead of up to four
 torch elementwise kernels.  On a stock `nn.BatchNorm2d` the same helper runs plain torch ops.
 """
 from __future__ import annotations
@@ -55,7 +55,7 @@ def conv_bn_act(conv: nn.Conv2d, bn: nn.Module, x: torch.Tensor, *, relu: bool =
                 residual: torch.Tensor | None = None) -> torch.Tensor:
     """y = act( BN( conv(x) [+ pre_conv(pre_x)] ) [+ residual] ) with `pre = (pre_conv, pre_x)`.
 
-    On the B200 engine the convolution biases are not added by a separate elementwise pass (and their gradients not
+    On the engine the convolution biases are not added by a separate elementwise pass (and their gradients not
     reduced by a separate kernel): the SyncBN kernel folds them in (`conv_bias=`) and its backward produces Σ dz."""
     fused = getattr(bn, "fused_forward", None)
     if fused is not None and x.is_cuda:
@@ -67,7 +67,7 @@ def conv_bn_act(conv: nn.Conv2d, bn: nn.Module, x: torch.Tensor, *, relu: bool =
 
 # torch.autocast lists upsample_bilinear2d as an fp32 op: under bf16 autocast every interpolate becomes
 # cast-up → fp32 kernel → fp32 result that then drags the following adds into fp32 (≈2 ms of casts per iteration on
-# the TestModel).  The B200 engine sets this flag so the interpolation runs natively in the activation dtype
+# the TestModel).  The engine sets this flag so the interpolation runs natively in the activation dtype
 # (the kernel still accumulates in fp32 internally; only the stored result is rounded to bf16).
 INTERPOLATE_IN_ACTIVATION_DTYPE = False
 
@@ -77,7 +77,7 @@ def bilinear(x: torch.Tensor, **kw) -> torch.Tensor:
     if len(kw) != 1 or next(iter(kw)) not in ("size", "scale_factor"):
         raise ValueError("bilinear() takes exactly one of size= / scale_factor=")
     if x.is_cuda:
-        from .. import resample                      # B200 engine: deterministic channels-last ×2 kernel
+        from .. import resample                      # engine: deterministic channels-last ×2 kernel
         out_hw = kw["size"] if "size" in kw else ((int(x.shape[2] * kw["scale_factor"]), int(x.shape[3] * kw["scale_factor"]))
                                                   if kw["scale_factor"] == 2 else None)
         if out_hw is not None:

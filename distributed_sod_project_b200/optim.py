@@ -165,7 +165,7 @@ def _same_physical_order(a: torch.Tensor, b: torch.Tensor) -> bool:
 
 
 class FusedSGD(Optimizer):
-    """SGD with momentum / weight decay as one flat sm_100a kernel; gradient averaging folded in when
+    """SGD with momentum / weight decay as one flat sm_90a kernel; gradient averaging folded in when
     distributed.  Arithmetic = torch.optim.SGD (torch/optim/sgd.py:343-380) with dampening 0, nesterov False."""
 
     def __init__(self, params, lr=1e-3, momentum=0.0, weight_decay=0.0, nesterov=False, model: nn.Module | None = None):
@@ -377,7 +377,7 @@ class FusedSGD(Optimizer):
         self.flat.refresh_shadow()
 
     def __repr__(self):
-        return super().__repr__().replace("FusedSGD", "FusedSGD[sm_100a flat]", 1)
+        return super().__repr__().replace("FusedSGD", "FusedSGD[sm_90a flat]", 1)
 
 
 def make_optimizer(model: nn.Module, optimizer_type: str, optimizer_info: dict) -> Optimizer:

@@ -13,8 +13,8 @@ import torch
 
 from . import _lib
 
-ENABLED = False     # switched on by the B200 engine (engine.Trainer)
-# the stem's MaxPool2d(3, 2, 1) through csrc/maxpool.cu (checked against torch on B200 in round 2; SOD_MAXPOOL=0 → torch op)
+ENABLED = False     # switched on by the engine (engine.Trainer)
+# the stem's MaxPool2d(3, 2, 1) through csrc/maxpool.cu (checked against torch by tests/test_gpu_resample.py; SOD_MAXPOOL=0 → torch op)
 MAXPOOL_ENABLED = os.environ.get("SOD_MAXPOOL", "1") == "1"
 # bias gradient of the convolutions that do not feed a BatchNorm as a deterministic column sum (SOD_COLSUM=0 → autograd's reduction)
 COLSUM_ENABLED = os.environ.get("SOD_COLSUM", "1") == "1"

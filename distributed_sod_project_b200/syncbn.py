@@ -33,8 +33,7 @@ def _launch_flags() -> int:
 
 FORCE_LOCAL = False         # bench.py roofline replay: run single-rank (no exchange) even inside a process group
 # BN+ReLU layers without a residual re-derive the ReLU mask from x in the backward instead of reading y (one input stream
-# less).  Default on since round 2: per-layer A/B on B200 (profiles/r02_call1_ab_bn_bwd.txt) 2531 → 2231 µs for the 84
-# backward launches together with the L2 hints, dz identical to the y-mask variant.  SOD_BN_MASK_FROM_X=0 turns it off.
+# less); dz is identical to the y-mask variant (tools/ab_bn_bwd_variants.py compares them).  SOD_BN_MASK_FROM_X=0 turns it off.
 MASK_FROM_X = os.environ.get("SOD_BN_MASK_FROM_X", "1") == "1"
 # L2 eviction-priority hints on the backward's bulk copies (same A/B; SOD_BN_L2_HINTS=0 turns them off)
 L2_HINTS = os.environ.get("SOD_BN_L2_HINTS", "1") == "1"
@@ -200,7 +199,7 @@ class SyncBatchNorm(nn.BatchNorm2d):
     def fused_forward(self, x, pre_add=None, residual=None, relu=False, conv_bias=(None, None)):
         """`conv_bias`: biases of the (bias-less) convolutions that produced `x` / `pre_add`, folded into the kernel"""
         if not x.is_cuda:
-            raise _lib.SodError("SyncBatchNorm: expected a CUDA tensor (the sm_100a kernel has no CPU fallback; "
+            raise _lib.SodError("SyncBatchNorm: expected a CUDA tensor (the sm_90a kernel has no CPU fallback; "
                                 "keep nn.BatchNorm2d for CPU runs)")
         if x.shape[1] != self.num_features:
             raise ValueError(f"expected {self.num_features} channels, got {x.shape[1]}")

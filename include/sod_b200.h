@@ -1,4 +1,4 @@
-/* sod_b200.h — C ABI of libsod_b200.so: the B200 (sm_100a) data-parallel hot path of
+/* sod_b200.h — C ABI of libsod_b200.so: the H100 (sm_90a) data-parallel hot path of
  * lartpang/Distributed-SOD-Project.
  *
  * The reference is pure Python and has NO FFI layer of its own (SURVEY §8b): its hot path is reached
@@ -43,7 +43,7 @@ enum {
 
 int sod_version(void);
 const char* sod_strerror(int code);
-/* sm count / compute capability of the current device; the hot path refuses anything but sm_100 */
+/* sm count / compute capability of the current device; the hot path refuses anything but sm_90 */
 int sod_device_info(int* sm_count, int* cc_major, int* cc_minor);
 
 /* ------------------------------------------------------------------------------------------------
@@ -226,7 +226,7 @@ int sod_colsum(const void* x, void* out, int64_t rows, int c, int dtype, void* w
  * backbone/origin/from_origin.py:7-15), channels-last [N,H,W,C], C % 8 == 0; (h, w) = INPUT size, output
  * ((h-1)/2+1, (w-1)/2+1).  argmax: one byte per OUTPUT element (window position kh*3+kw), written by the forward and
  * read by the backward, which is a deterministic gather with fp32 accumulation.  Ties / NaN as torch: first maximum
- * in (kh, kw) scan order, NaN propagates.  (Checked against torch on B200 in round 2 and enabled by default.) */
+ * in (kh, kw) scan order, NaN propagates.  (Checked against torch by the GPU tests and enabled by default.) */
 int sod_maxpool3x3s2_fwd(const void* x, void* y, void* argmax, int n, int h, int w, int c, int dtype, void* stream);
 int sod_maxpool3x3s2_bwd(const void* dy, const void* argmax, void* dx, int n, int h, int w, int c, int dtype, void* stream);
 

@@ -9,10 +9,10 @@ Parity status
 * Reference-owned arithmetic (`loss/CEL.py:15-20`, `BCEWithLogitsLoss` at `train.py:203`,
   `utils/pipeline_ops.py` `get_total_loss` 19-43 / `CustomScheduler` 185-232 / `make_optimizer` 235-316,
   `utils/tensor_ops.py:60-64`, `network/TestModel.py`) is PINNED: `tools/make_golden.py` imports the
-  unmodified reference modules from /root/reference in the build container and writes
+  unmodified reference modules from a checkout of the reference and writes
   `tests/golden/*.npz`; `tests/test_oracle_golden.py` checks every oracle function against them.
 * The apex pieces (`apex.parallel.DistributedDataParallel`, `apex.parallel.SyncBatchNorm`, `apex.amp`;
-  call sites `train.py:15-16,180-185,299`) are NOT in /root/reference (un-vendored, un-pinned:
+  call sites `train.py:15-16,180-185,299`) are NOT in the reference repository (un-vendored, un-pinned:
   `readme.md:40-42`) and apex is not installed here: **parity unpinned** for those.  Their published
   semantics are restated here and cross-checked against the equivalent single-process computation
   (W-rank SyncBN+DDP == one process on the concatenated batch, see `oracle/syncbn.py`) and, on the GPU

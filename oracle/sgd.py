@@ -7,7 +7,7 @@ Follows
   configured by the reference `make_optimizer(..., "f3_trick")` — utils/pipeline_ops.py:295-313
   (backbone lr×0.1, head lr×1, names starting with `div_2` in no group), stepped at train.py:303;
 * apex `DistributedDataParallel(delay_allreduce=True)` published semantics (train.py:185): one flat
-  buffer, SUM all-reduce, then ×1/world_size (parity unpinned — apex is not in /root/reference);
+  buffer, SUM all-reduce, then ×1/world_size (parity unpinned — apex is not in the reference repository);
 * apex `amp.scale_loss` exit: grads ×1/S, step skipped if any grad is non-finite (train.py:299).
 * `CustomScheduler` — utils/pipeline_ops.py:185-232.
 

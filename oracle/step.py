@@ -14,7 +14,7 @@ and the apex wrappers by their published semantics: SyncBN = batch statistics ov
 the stock torch module refuses CPU tensors, torch/nn/modules/batchnorm.py:798-811).
 
 `model_factory` is injected: tools/make_golden.py passes the UNMODIFIED reference `network.res50`
-(imported from /root/reference in the build container); the GPU box passes this repo's plugin of the
+(imported from a checkout of the reference); tests and bench.py pass this repo's plugin of the
 same architecture (bit-identical init and outputs: tests/test_host_cpu.py::test_model_plugin_is_bit_identical_to_reference).
 """
 from __future__ import annotations

@@ -1,7 +1,7 @@
 """ORACLE (test infrastructure only): synchronized batch-norm over W ranks, numpy fp64.
 
 Restates the published semantics of `apex.parallel.SyncBatchNorm` as installed by
-`convert_syncbn_model` (reference train.py:180; apex itself is NOT under /root/reference —
+`convert_syncbn_model` (reference train.py:180; apex itself is NOT in the reference repository —
 **parity unpinned**), using the readable in-container equivalent as the arithmetic spec:
 torch/nn/modules/_functions.py:7-209 (`SyncBatchNorm`): training statistics are taken over
 N·H·W of ALL ranks (equal per-rank counts here), running_mean/var use momentum 0.1 with the

@@ -128,11 +128,15 @@ def test_rejects_cpu_and_misuse():
         bce_cel_fwd_bwd(torch.zeros(4, device="cuda"), torch.zeros(5, device="cuda"))
 
 
-@pytest.mark.parametrize("n", [4096 * 3 + 5, 148 * 4096 * 9, 148 * 4096 * 10 + 777, 148 * 4096 * 23 + 8, 33_000_001])
-@pytest.mark.parametrize("dtype", [torch.float32, torch.bfloat16])
-def test_ring_streamed_kernel_matches_oracle(n, dtype):
-    """mode 2 forces the ring-streamed kernel (producer warp + shared-memory ring, re-stream newest first): fewer chunks
-    than stages (nothing re-streamed), exactly as many, one more, many more, and a ragged scalar tail"""
+def _sm_count() -> int:
+    import ctypes
+    from distributed_sod_project_b200 import _lib
+    sms = ctypes.c_int(0)
+    _lib.check(_lib.lib().sod_device_info(ctypes.byref(sms), None, None), "sod_device_info")
+    return sms.value
+
+
+def _check_ring_streamed(n, dtype):
     from distributed_sod_project_b200.loss import bce_cel_fwd_bwd
     gcpu = torch.Generator().manual_seed(n % 1000)
     x = (torch.randn(n, generator=gcpu) * 3).to(dtype)
@@ -147,3 +151,21 @@ def test_ring_streamed_kernel_matches_oracle(n, dtype):
     assert np.abs(gr - ref["grad"]).max() / scale < tol
     resident, _ = bce_cel_fwd_bwd(x.cuda(), t.cuda(), mode=0)
     assert resident.cpu().numpy()[2] == pytest.approx(s[2], rel=1e-6)
+
+
+@pytest.mark.parametrize("n", [4096 * 3 + 5, 148 * 4096 * 9, 148 * 4096 * 10 + 777, 148 * 4096 * 23 + 8, 33_000_001])
+@pytest.mark.parametrize("dtype", [torch.float32, torch.bfloat16])
+def test_ring_streamed_kernel_matches_oracle(n, dtype):
+    """mode 2 forces the ring-streamed kernel (producer warp + shared-memory ring, re-stream newest first) at fixed sizes,
+    including a ragged scalar tail"""
+    _check_ring_streamed(n, dtype)
+
+
+# n = chunks_per_sm * #SMs * 4096 + extra: one CTA per SM, 4096-element chunks, so the chunk count per CTA does not depend
+# on how many SMs the device has
+@pytest.mark.parametrize("chunks_per_sm, extra", [(9, 0), (10, 777), (23, 8)])
+@pytest.mark.parametrize("dtype", [torch.float32, torch.bfloat16])
+def test_ring_streamed_kernel_chunks_per_cta(chunks_per_sm, extra, dtype):
+    """the ring-streamed kernel with the same number of chunks per CTA on any device: fewer chunks than stages (nothing
+    re-streamed), exactly as many, one more, many more"""
+    _check_ring_streamed(chunks_per_sm * _sm_count() * 4096 + extra, dtype)

@@ -1,5 +1,5 @@
 """World-size-2 parity of the peer-memory collectives (needs ≥2 GPUs on one NVSwitch domain; skipped otherwise).
-Run with `gpurun --gpus 2 -- python -m pytest tests/test_gpu_multi.py -m gpu`."""
+Run on a machine with at least two GPUs: `python -m pytest tests/test_gpu_multi.py -m gpu`."""
 import os
 import socket
 

@@ -29,6 +29,11 @@ def test_fp32_trajectory_vs_reference(golden, tag, model):
         # deepest BN) are an ill-conditioned edge case whose later iterations amplify fp32 reassociation noise —
         # the oracle itself moves by 3e-3 at iteration 1 between a 1-process and a 2-process run (DESIGN.md §parity)
         well = tag.endswith("s128")
+        if well and it >= 2:
+            # from iteration 2 on the reference's own float32 run is 2e-3 away from its float64 run here
+            # (tools/diag_reference_fp64.py 4 128), so the float32 golden value is one sample of that noise: hold the loss
+            # to the float64 trajectory of the reference instead (tools/make_golden.py --only-fp64)
+            ref = float(golden(f"step_{tag}_fp64.npz")[f"loss{it}"][0])
         if well or it == 0:
             assert out["loss"] == pytest.approx(ref, rel=1e-3 if it < 2 else 5e-3), f"iter {it}: got {out['loss']} want {ref}"
         else:   # ill-conditioned edge case: later iterations only have to stay in the neighbourhood (run-to-run chaos)
@@ -62,7 +67,7 @@ def test_fp32_trajectory_vs_reference(golden, tag, model):
 
 
 def test_bf16_first_step_within_tolerance(golden):
-    """BASELINE config-1 shape (bs 4, 320²) in the B200 configuration (bf16 autocast, channels-last)."""
+    """BASELINE config-1 shape (bs 4, 320²) in the benchmark configuration (bf16 autocast, channels-last)."""
     from distributed_sod_project_b200.synthetic import synth_batch
     g = golden("step_res50_w1_s320.npz")
     tr = _trainer("res50", dtype=torch.bfloat16, channels_last=True)
@@ -187,7 +192,7 @@ def test_step_from_host_feeds_every_batch(prefetch, monkeypatch):
 
 @pytest.mark.parametrize("tag,bs", [("res50_w1_s320", 4), ("res50_w1_s320_bs16", 16)])
 def test_fp32_benched_configuration_loss_and_logits(golden, tag, bs):
-    """The configuration bench.py times (320², bs 4 = BASELINE config 1 and bs 16 = the B200 batch) against the
+    """The configuration bench.py times (320², bs 4 = BASELINE config 1 and bs 16 = the benched batch) against the
     UNMODIFIED reference in fp32: north_star's 1e-3 relative on the loss (iterations 0 and 1) AND on the per-pixel
     logits of iteration 0 (stored spatially subsampled, tools/make_golden.py).
     Iteration-1 logits are a different matter: they are the output of the network AFTER the first SGD step, and the

@@ -1,4 +1,4 @@
-"""The reference's command line (`python train.py -ng N`) drives the B200 engine end to end."""
+"""The reference's command line (`python train.py -ng N`) drives the engine end to end."""
 import json
 import os
 import subprocess

@@ -91,7 +91,7 @@ def test_model_matches_torch(h, w, kind):
 def test_cpu_tensors_keep_the_torch_op():
     from distributed_sod_project_b200 import resample
     from distributed_sod_project_b200.network import blocks
-    assert resample.MAXPOOL_ENABLED is True        # default on since the round-2 hardware check (profiles/r02_call1_*)
+    assert resample.MAXPOOL_ENABLED is True        # default on: checked against torch by tests/test_gpu_resample.py
     pool = blocks._StemPool(3, 2, 1)
     x = torch.randn(1, 8, 6, 6)
     assert torch.equal(pool(x), F.max_pool2d(x, 3, 2, 1))                   # CPU / disabled → torch op

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """How well-conditioned is "per-pixel logits of iteration 1"?  Runs the UNMODIFIED reference model / loss / optimizer
-(/root/reference, CPU) twice on the same seeded inputs — once in float32 (what the golden vectors hold) and once in
+(SOD_REFERENCE, CPU) twice on the same seeded inputs — once in float32 (what the golden vectors hold) and once in
 float64 — and prints the distance between the two trajectories.  The float64 run is the exact-arithmetic proxy: whatever
 separates it from the float32 run is rounding noise of the REFERENCE ITSELF, i.e. the floor below which no other
 implementation can be compared with the float32 golden vectors.  (Build container only; output committed under

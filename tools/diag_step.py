@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""GPU-box diagnostic: per-parameter gradient error of iteration 0 (fp32) of the B200 engine vs the CPU oracle
+"""GPU-box diagnostic: per-parameter gradient error of iteration 0 (fp32) of the engine vs the CPU oracle
 trainer, with this repo's SyncBN kernels and, for attribution, with stock torch BatchNorm on the GPU."""
 import os, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))

@@ -1,9 +1,9 @@
 #!/usr/bin/env python
-"""Generate tests/golden/*.npz by running the UNMODIFIED reference (/root/reference) on CPU.
+"""Generate tests/golden/*.npz by running the UNMODIFIED reference on CPU.
 
-Run in the build container only (the GPU box has no /root/reference):
+Needs a checkout of lartpang/Distributed-SOD-Project; the tests only read the committed vectors:
 
-    python tools/make_golden.py
+    SOD_REFERENCE=/path/to/Distributed-SOD-Project python tools/make_golden.py [--only-320 | --only-model-init | --only-fp64]
 
 The reference modules are imported as they are; three `sys.modules` shims stand in for packages that
 are missing / removed in this image and that the hot path never calls (SURVEY §8c):
@@ -11,7 +11,7 @@ are missing / removed in this image and that the hot path never calls (SURVEY §
 `torch.utils.model_zoo.load_url` returns {} (no network: backbone/origin/resnet.py:208-215 then keeps
 the seeded random init).
 
-apex (DDP / SyncBN / amp) is not part of /root/reference, so the W=2 vectors are produced from the
+apex (DDP / SyncBN / amp) is not part of the reference repository, so the W=2 vectors are produced from the
 reference's own model / loss / optimizer with apex's published semantics restated as the equivalent
 single-process computation: SyncBN over W ranks == BatchNorm over the rank-concatenated batch, and
 the DDP gradient mean == gradient of mean_r(loss_r).  (Parity unpinned for apex itself.)
@@ -29,13 +29,13 @@ REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, REPO)
 from distributed_sod_project_b200.synthetic import synth_batch  # noqa: E402
 
-REF = "/root/reference"
+REF = os.environ.get("SOD_REFERENCE", "")
 OUT = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests", "golden")
 
 
 def install_reference():
     if not os.path.isdir(REF):
-        raise SystemExit("reference not present; golden vectors can only be regenerated in the build container")
+        raise SystemExit("set SOD_REFERENCE to a checkout of the reference to regenerate the golden vectors")
     sys.path.insert(0, REF)
     m = types.ModuleType("torchvision.models.utils")
     m.load_state_dict_from_url = lambda *a, **k: {}
@@ -152,21 +152,23 @@ def _probe_params(model):
     return {k: sd[k].detach().reshape(-1)[:64].numpy().copy() for k in keys}
 
 
-def step_vectors(model_name: str, world: int, bs: int, size: int, iters: int, tag: str, keep_logits=(0,), logits_stride: int = 1):
-    """reference model + reference loss/optimizer, apex semantics restated (see module docstring)."""
+def step_vectors(model_name: str, world: int, bs: int, size: int, iters: int, tag: str, keep_logits=(0,), logits_stride: int = 1,
+                 dtype=torch.float32):
+    """reference model + reference loss/optimizer, apex semantics restated (see module docstring).  dtype=float64 gives
+    the arithmetic the float32 vectors are rounding noise around (later iterations of a trajectory are compared with it)."""
     import network
     from loss.CEL import CEL
     from utils.misc import init_seed
     from utils.pipeline_ops import get_total_loss, make_optimizer
     init_seed(0)
-    model = getattr(network, model_name)()
+    model = getattr(network, model_name)().to(dtype)
     opt = make_optimizer(model, "f3_trick", dict(lr=0.05, momentum=0.9, weight_decay=5e-4, nesterov=False))
     loss_funcs = [torch.nn.BCEWithLogitsLoss(reduction="mean"), CEL()]
     model.train()
     out = {"meta": np.array([world, bs, size, iters]), "logits_stride": np.array(logits_stride)}
     for it in range(iters):
         batches = [synth_batch(1234 + r + 1000 * it, bs, size) for r in range(world)]
-        x = torch.cat([b[0] for b in batches]); m = torch.cat([b[1] for b in batches])
+        x = torch.cat([b[0] for b in batches]).to(dtype); m = torch.cat([b[1] for b in batches]).to(dtype)
         preds = model(x)                                   # BN over the concatenated batch == SyncBN
         per_rank, strs = [], []
         for r in range(world):
@@ -188,10 +190,38 @@ def step_vectors(model_name: str, world: int, bs: int, size: int, iters: int, ta
     np.savez_compressed(os.path.join(OUT, f"step_{tag}.npz"), **out)
 
 
+def model_init_vectors(model_name: str = "res50", samples: int = 32):
+    """the reference model right after `init_seed(0)`: every state_dict key and shape, per-tensor float64 sum and sum of
+    squares, a fixed seeded sample of values per tensor, and the output of one forward pass on a seeded input
+    (tests/test_host_cpu.py::test_model_plugin_is_bit_identical_to_reference compares the package's plugin with it)"""
+    import network
+    from utils.misc import init_seed
+    init_seed(0)
+    model = getattr(network, model_name)()
+    sd = model.state_dict()
+    shapes, vals, moments = [], [], []
+    for v in sd.values():
+        a = v.detach().reshape(-1).double().numpy()
+        idx = np.linspace(0, a.size - 1, samples).astype(np.int64)      # the same positions are recomputed by the test
+        shapes.append(list(v.shape) + [-1] * (4 - v.dim()))
+        vals.append(a[idx])
+        moments.append([a.sum(), (a * a).sum()])
+    x = torch.randn(2, 3, 64, 64, generator=torch.Generator().manual_seed(0))
+    out = {"keys": np.array("\n".join(sd)), "shapes": np.array(shapes, dtype=np.int64), "values": np.array(vals),
+           "moments": np.array(moments), "x": x.numpy(), "y": model(x).detach().numpy()}
+    np.savez_compressed(os.path.join(OUT, f"model_{model_name}_init.npz"), **out)
+
+
 def main():
     os.makedirs(OUT, exist_ok=True)
     install_reference()
     torch.set_num_threads(8)
+    if "--only-model-init" in sys.argv:
+        model_init_vectors()
+        return
+    if "--only-fp64" in sys.argv:
+        step_vectors("res50", 1, 4, 128, 3, "res50_w1_s128_fp64", keep_logits=(), dtype=torch.float64)
+        return
     if "--only-320" in sys.argv:      # round 2: the benched configuration pinned with logits (bs 4 and bs 16 at 320x320)
         step_vectors("res50", 1, 4, 320, 3, "res50_w1_s320", keep_logits=(0, 1), logits_stride=2)
         step_vectors("res50", 1, 16, 320, 2, "res50_w1_s320_bs16", keep_logits=(0, 1), logits_stride=4)
@@ -204,6 +234,7 @@ def main():
     step_vectors("cp_res50", 1, 2, 64, 3, "cp_res50_w1_s64", keep_logits=(0,))
     step_vectors("res50", 2, 2, 64, 4, "res50_w2_s64", keep_logits=(0, 3))
     step_vectors("res50", 1, 4, 128, 4, "res50_w1_s128", keep_logits=(0,))
+    step_vectors("res50", 1, 4, 128, 3, "res50_w1_s128_fp64", keep_logits=(), dtype=torch.float64)
     step_vectors("res50", 2, 4, 128, 4, "res50_w2_s128", keep_logits=(0,))
     step_vectors("res50", 1, 4, 320, 3, "res50_w1_s320", keep_logits=(0, 1), logits_stride=2)   # BASELINE config 1 shape
     step_vectors("res50", 1, 16, 320, 2, "res50_w1_s320_bs16", keep_logits=(0, 1), logits_stride=4)   # the benched batch size

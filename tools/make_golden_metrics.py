@@ -1,16 +1,16 @@
 #!/usr/bin/env python
 """Golden vectors for the evaluation metrics, produced by the UNMODIFIED reference classes
-(/root/reference/utils/saliency_metric.py: CalTotalMetric and its five Cal* members) on seeded synthetic
+(utils/saliency_metric.py of the reference: CalTotalMetric and its five Cal* members) on seeded synthetic
 prediction / ground-truth pairs normalised exactly as the reference's test loop does (train.py:396-409).
-Writes tests/golden/metrics_kat.npz (inputs as uint8, per-image terms and the dataset dict).  Runs in the build
-container only (needs /root/reference); the committed .npz is what travels."""
+Writes tests/golden/metrics_kat.npz (inputs as uint8, per-image terms and the dataset dict).  Needs a checkout of the
+reference (SOD_REFERENCE=/path/to/Distributed-SOD-Project); the tests only read the committed .npz."""
 import os
 import sys
 
 import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, "/root/reference")
+sys.path.insert(0, os.environ["SOD_REFERENCE"])
 from utils.saliency_metric import CalTotalMetric  # noqa: E402
 
 

@@ -1,5 +1,5 @@
-// membench.cu — B200 streaming-read microbenchmark used to choose the SyncBN staging scheme (tools only).
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o membench membench.cu && ./membench
+// membench.cu — streaming-read microbenchmark used to choose the SyncBN staging scheme (tools only).
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o membench membench.cu && ./membench
 #include <cuda_runtime.h>
 #include <cstdio>
 #include <cstdint>

@@ -10,7 +10,7 @@ TMP=$(mktemp -d)
 {
   echo "# ptxas -v (registers / spills / smem per kernel), nvcc $(nvcc --version | grep -o 'V[0-9]*\.[0-9]*\.[0-9]*')"
   for f in loss sgd syncbn resample maxpool pipeline api; do
-    nvcc -gencode arch=compute_100a,code=sm_100a -O3 -lineinfo -std=c++17 -Iinclude -Xptxas=-v \
+    nvcc -gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -std=c++17 -Iinclude -Xptxas=-v \
          -c distributed_sod_project_b200/csrc/$f.cu -o $TMP/$f.o 2>&1 \
       | c++filt | awk '/Compiling entry function/ {name=$0; sub(/.*function ./,"",name); sub(/. for.*/,"",name)}
                        /bytes spill/ {sp=""; if ($0 !~ / 0 bytes spill stores, 0 bytes spill loads/) {sp=$0; sub(/^ */,"",sp)}}

@@ -5,7 +5,7 @@
 
 Same process model as the reference (`torch.multiprocessing.spawn`, one process per GPU, env:// rendezvous,
 train.py:84-101) and the same construction order in `main_worker` (train.py:104-223); the hot path is this repo's
-B200 engine (`distributed_sod_project_b200/engine.py`).  NCCL is still initialised — it bootstraps the symmetric-memory
+engine (`distributed_sod_project_b200/engine.py`).  NCCL is still initialised — it bootstraps the symmetric-memory
 rendezvous — but no NCCL collective runs inside an iteration.
 
 Out of scope here (SURVEY §2): TensorBoard / xlsx recorders, dataset decoding.  Evaluation (`test`, `_test_process`) runs
@@ -31,7 +31,7 @@ from distributed_sod_project_b200.synthetic import synth_batch, synth_eval_set
 from distributed_sod_project_b200.utils import (AvgMeter, check_mkdir, construct_exp_name, construct_path_dict, construct_print,
                                                 init_cudnn, write_data_to_file)
 
-parser = argparse.ArgumentParser(prog="main script", description="B200-native engine behind the Distributed-SOD-Project API.",
+parser = argparse.ArgumentParser(prog="main script", description="H100-native engine behind the Distributed-SOD-Project API.",
                                  allow_abbrev=False)
 parser.version = "1.0.0"
 parser.add_argument("-v", "--version", action="version")
