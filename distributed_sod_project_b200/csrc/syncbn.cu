@@ -889,8 +889,18 @@ __device__ __forceinline__ void store8_hint(T* p, const float (&f)[8], uint64_t 
 
 // XMASK (experimental, SOD_BN_BWD_MASK_FROM_X): a BN+ReLU layer without residual does not stream y at all — the
 // mask y > 0 is re-derived from x with the forward's own arithmetic (y = fma(z, invstd*γ, fma(b, invstd*γ, β - mean*invstd*γ)),
-// same operations in the same order, so the sign agrees with the stored y except where |y| is denormal).  One stream
-// less to read twice: compulsory bytes drop from 4 to 3 tensors, and a third more of the strip stays resident.
+// same operations in the same order, so the sign agrees with the stored y; for bf16 except where |y| is below the
+// smallest bf16 denormal, for fp16 see stored_positive).  One stream less to read twice: compulsory bytes drop from 4
+// to 3 tensors, and a third more of the strip stays resident.
+//
+// y > 0 as the forward STORED it: an fp16 store rounds every fp32 y in (0, 2^-25] to +0, where torch's relu (and the
+// y-mask variant) pass no gradient, so the fp16 sign is taken after the same rounding.
+template <typename T>
+__device__ __forceinline__ bool stored_positive(float y) {
+    if constexpr (std::is_same<T, __half>::value) return __half2float(__float2half_rn(y)) > 0.f;
+    else return y > 0.f;
+}
+
 template <typename T, int NSTAT, bool XMASK = false, bool HINT = false>
 __global__ void __launch_bounds__(kBlock, 1) syncbn_bwd_kernel(const __grid_constant__ BnBwd prm) {
     extern __shared__ __align__(128) unsigned char smem[];
@@ -972,7 +982,7 @@ __global__ void __launch_bounds__(kBlock, 1) syncbn_bwd_kernel(const __grid_cons
         }
         if (XMASK) {
 #pragma unroll
-            for (int k = 0; k < 8; ++k) d[k] = fmaf(z[k], msc[XMASK ? k : 0], msh[XMASK ? k : 0]) > 0.f ? d[k] : 0.f;
+            for (int k = 0; k < 8; ++k) d[k] = stored_positive<T>(fmaf(z[k], msc[XMASK ? k : 0], msh[XMASK ? k : 0])) ? d[k] : 0.f;
         } else if (relu) {
             float o[8];
             IO<T>::load8(reinterpret_cast<const T*>(ring.buf(s, k_y)) + q * 8, o);

@@ -31,6 +31,11 @@ def test_preprocess_batch_matches_the_reference_transforms(hs, ws, size, with_ma
     xb, _ = preprocess_batch(img.cuda(), mask.cuda() if with_mask else None, size=size, flip=flip.cuda() if with_flip else None,
                              dtype=torch.bfloat16)
     assert xb.dtype == torch.bfloat16 and float((xb.float().cpu() - want_x).abs().max()) <= 2.0 ** -7 * float(want_x.abs().max())
+    # fp16 (the apex O1 input dtype): the fp32 value above rounded once, so within one fp16 ulp of the reference plus its 4e-6
+    xh, _ = preprocess_batch(img.cuda(), mask.cuda() if with_mask else None, size=size, flip=flip.cuda() if with_flip else None,
+                             dtype=torch.float16)
+    ulp16 = torch.exp2(torch.floor(torch.log2(want_x.double().abs().clamp_min(2.0 ** -14))) - 10)
+    assert xh.dtype == torch.float16 and bool(((xh.double().cpu() - want_x.double()).abs() <= ulp16 + 4e-6).all())
 
 
 def test_device_prefetcher_yields_every_batch_in_order():

@@ -189,8 +189,8 @@ def test_folded_conv_bias(shape, dtype, bdtype, two):
 @pytest.mark.parametrize("dtype", [torch.float32, torch.bfloat16])
 @pytest.mark.parametrize("with_pre,with_cb", [(False, False), (True, False), (False, True)])
 @pytest.mark.parametrize("hints", [False, True])
-def test_bwd_mask_from_x_agrees_with_mask_from_y(shape, dtype, with_pre, with_cb, hints):
-    """SOD_BN_BWD_MASK_FROM_X re-derives the ReLU mask from x: against the default variant on the same inputs the result
+def test_bwd_mask_from_x_agrees_with_mask_from_y(shape, dtype, with_pre, with_cb, hints, monkeypatch):
+    """SOD_BN_BWD_MASK_FROM_X re-derives the ReLU mask from x: against the y-mask variant on the same inputs the result
     may differ only by the summation order of the statistics (different strip geometry)."""
     from distributed_sod_project_b200 import syncbn
     n, c, h, w = shape
@@ -203,14 +203,12 @@ def test_bwd_mask_from_x_agrees_with_mask_from_y(shape, dtype, with_pre, with_cb
     dy = _mk(shape, dtype, 4)
     out = {}
     for flag in (False, True):
-        syncbn.MASK_FROM_X, syncbn.L2_HINTS = flag, hints and flag
-        try:
-            dcb = (torch.zeros_like(cb[0]), None) if with_cb else (None, None)
-            dz, _, dg, db = syncbn.raw_backward(dy, x.detach(), pre, y.detach(), bn.weight.detach(), mean, invstd, True, False,
-                                                conv_bias=tuple(None if t is None else t.detach() for t in cb),
-                                                dconv_bias=dcb, bias=bn.bias.detach())
-        finally:
-            syncbn.MASK_FROM_X, syncbn.L2_HINTS = False, False
+        monkeypatch.setattr(syncbn, "MASK_FROM_X", flag)       # restored to the session's setting when the test ends
+        monkeypatch.setattr(syncbn, "L2_HINTS", hints and flag)
+        dcb = (torch.zeros_like(cb[0]), None) if with_cb else (None, None)
+        dz, _, dg, db = syncbn.raw_backward(dy, x.detach(), pre, y.detach(), bn.weight.detach(), mean, invstd, True, False,
+                                            conv_bias=tuple(None if t is None else t.detach() for t in cb),
+                                            dconv_bias=dcb, bias=bn.bias.detach())
         torch.cuda.synchronize()
         out[flag] = (dz.float(), dg, db, None if dcb[0] is None else dcb[0].float())
     scale = float(out[False][0].abs().max())
