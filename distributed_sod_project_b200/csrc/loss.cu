@@ -3,12 +3,12 @@
 // Reference arithmetic: torch.nn.BCEWithLogitsLoss (reference train.py:203) + CEL.forward
 // (reference loss/CEL.py:15-20) summed by get_total_loss (reference utils/pipeline_ops.py:37-42).
 //
-// The CEL gradient of every pixel needs three sums over the WHOLE tensor (Σp, Σt, Σp·t), so a plain
+// The CEL gradient of every pixel needs three sums over the WHOLE tensor (Σp, Σt, Σd), so a plain
 // elementwise kernel cannot emit gradients in the pass that reads the logits.  Design:
 //   * one CTA per SM (cooperative launch), each owning a contiguous slice of the tensor;
 //   * the slice is pulled into shared memory with 1-D bulk async copies (TMA engine, mbarrier
 //     completion) in 4096-element chunks so compute on chunk 0 overlaps the arrival of chunk k;
-//   * phase 1 reduces (Σbce, Σp, Σt, Σpt) from shared memory → per-CTA partial → grid barrier →
+//   * phase 1 reduces (Σbce, Σp, Σt, Σd) from shared memory (d: see Sums) → per-CTA partial → grid barrier →
 //     every CTA re-reduces the per-CTA partials (one per SM) in the same fixed order (deterministic, no atomics);
 //   * phase 2 re-reads the slice FROM SHARED MEMORY and writes the gradient: logits and mask cross
 //     HBM exactly once (8 B/elem algorithmic with bf16 logits + fp32 mask + bf16 grad).
@@ -38,25 +38,37 @@ struct LossParams {
     float w_bce, w_cel, grad_scale, eps;
 };
 
+// d = p(1-t) + t(1-p) = |p - t| for a binary t: CEL's numerator term.  It is summed as such, never formed as
+// Σp + Σt - 2Σpt, which cancels when the predictions are confident and p ≈ t (late in training).
 struct Sums {
-    float bce, p, t, pt;
+    float bce, p, t, d;
 };
 
-__device__ __forceinline__ void loss_terms(float x, float t, Sums& s) {
+// p = sigmoid(x) and q = 1 - p, each from e = exp(-|x|) without a subtraction (1 - p loses q when q < ulp(1)); returns e
+__device__ __forceinline__ float sigmoid_pq(float x, float& p, float& q) {
     const float e = __expf(-fabsf(x));
     const float r = __fdividef(1.0f, 1.0f + e);
-    const float p = x >= 0.0f ? r : e * r;
-    s.bce += fmaxf(x, 0.0f) - x * t + __logf(1.0f + e);
+    p = x >= 0.0f ? r : e * r;
+    q = x >= 0.0f ? e * r : r;
+    return e;
+}
+
+__device__ __forceinline__ void loss_terms(float x, float t, Sums& s) {
+    float p, q;
+    const float e = sigmoid_pq(x, p, q);
+    // log1pf, not __logf(1 + e): that is off by up to 2^-21.4 absolute, 1 % of the whole term at |x| = 10
+    s.bce += fmaxf(x, 0.0f) - x * t + log1pf(e);
     s.p += p;
     s.t += t;
-    s.pt += p * t;
+    s.d += fmaf(p, 1.0f - t, t * q);
 }
 
 __device__ __forceinline__ float loss_grad(float x, float t, float kb, float alpha, float beta) {
-    const float e = __expf(-fabsf(x));
-    const float r = __fdividef(1.0f, 1.0f + e);
-    const float p = x >= 0.0f ? r : e * r;
-    // kb*(p - t) + p(1-p) * ((1-2t)*alpha + beta); alpha/beta already carry w_cel*grad_scale
+    float p, q;
+    sigmoid_pq(x, p, q);
+    // kb*(p - t) + p(1-p) * ((1-2t)*alpha + beta); alpha/beta already carry w_cel*grad_scale.  p - t and 1 - p are
+    // subtractions, as in the reference's autograd (sigmoid(x) - t): one fp32 ulp of 1 absolute.  Forming them from q
+    // instead rounds every gradient differently, and a training run drifts away from the reference's trajectory.
     return kb * (p - t) + p * (1.0f - p) * fmaf(1.0f - 2.0f * t, alpha, beta);
 }
 
@@ -129,7 +141,7 @@ __global__ void __launch_bounds__(kThreads, 1) loss_bce_cel_kernel(const LossPar
 
     // block reduce (fixed order) → one partial per CTA
     {
-        const float a = warp_sum(acc.bce), b = warp_sum(acc.p), c2 = warp_sum(acc.t), d = warp_sum(acc.pt);
+        const float a = warp_sum(acc.bce), b = warp_sum(acc.p), c2 = warp_sum(acc.t), d = warp_sum(acc.d);
         if ((tid & 31) == 0) {
             s_red[tid >> 5][0] = a; s_red[tid >> 5][1] = b; s_red[tid >> 5][2] = c2; s_red[tid >> 5][3] = d;
         }
@@ -155,8 +167,8 @@ __global__ void __launch_bounds__(kThreads, 1) loss_bce_cel_kernel(const LossPar
         if (tid == 0) { s_tot[0] = a; s_tot[1] = b; s_tot[2] = c2; s_tot[3] = d; }
     }
     __syncthreads();
-    const double bce_sum = s_tot[0], sp = s_tot[1], st = s_tot[2], spt = s_tot[3];
-    const double num = sp + st - 2.0 * spt;
+    const double bce_sum = s_tot[0], sp = s_tot[1], st = s_tot[2], num = s_tot[3];
+    const double spt = 0.5 * (sp + st - num);   // reported only: Σp·t = (Σp + Σt - Σd) / 2
     const double den = sp + st + static_cast<double>(prm.eps);
     const double cel = num / den;
     const double bce = prm.reduction_sum ? bce_sum : bce_sum / static_cast<double>(n);
@@ -298,7 +310,7 @@ __global__ void __launch_bounds__(kStreamBlock, 1) loss_stream_kernel(const Loss
     if (blockIdx.x == 0 && tid < ntail)
         loss_terms(IO<TX>::load1(gx + nvec + tid), IO<TM>::load1(gm + nvec + tid), acc);
     {
-        const float a = warp_sum(acc.bce), b = warp_sum(acc.p), c2 = warp_sum(acc.t), d = warp_sum(acc.pt);
+        const float a = warp_sum(acc.bce), b = warp_sum(acc.p), c2 = warp_sum(acc.t), d = warp_sum(acc.d);
         if ((tid & 31) == 0) { s_red[tid >> 5][0] = a; s_red[tid >> 5][1] = b; s_red[tid >> 5][2] = c2; s_red[tid >> 5][3] = d; }
         asm volatile("bar.sync 1, 512;" ::: "memory");
         if (tid == 0) {
@@ -318,8 +330,8 @@ __global__ void __launch_bounds__(kStreamBlock, 1) loss_stream_kernel(const Loss
         if (tid == 0) { s_tot[0] = a; s_tot[1] = b; s_tot[2] = c2; s_tot[3] = d; }
     }
     asm volatile("bar.sync 1, 512;" ::: "memory");
-    const double bce_sum = s_tot[0], sp = s_tot[1], st = s_tot[2], spt = s_tot[3];
-    const double num = sp + st - 2.0 * spt;
+    const double bce_sum = s_tot[0], sp = s_tot[1], st = s_tot[2], num = s_tot[3];
+    const double spt = 0.5 * (sp + st - num);   // reported only: Σp·t = (Σp + Σt - Σd) / 2
     const double den = sp + st + static_cast<double>(prm.eps);
     const double cel = num / den;
     const double bce = prm.reduction_sum ? bce_sum : bce_sum / static_cast<double>(n);
