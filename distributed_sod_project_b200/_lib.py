@@ -16,6 +16,7 @@ SOD_MAX_WORLD = 8
 SOD_MAX_SEGMENTS = 16
 SOD_SEG_FROZEN = 1
 SOD_SEG_GRAD16 = 2
+SOD_SEG_NESTEROV = 4
 SOD_SGD_ZERO_GRAD = 1
 SOD_ALGO_NO_MULTIMEM = 2
 SOD_BN_ACCUMULATE_PARAM_GRADS = 8
@@ -25,6 +26,7 @@ SOD_BN_L2_HINTS = 64
 SOD_BN_LAUNCH_COOP = 128
 SOD_BN_LAUNCH_PDL = 256
 SOD_GATHER_MAX_ITEMS = 160
+SOD_ADAM_STEP_WORDS = SOD_MAX_SEGMENTS + 1
 ABI_VERSION = 7
 
 
@@ -47,6 +49,11 @@ class sod_sgd_segment(C.Structure):
                 ("momentum", C.c_float), ("flags", C.c_int32)]
 
 
+class sod_adam_segment(C.Structure):
+    _fields_ = [("begin", C.c_int64), ("end", C.c_int64), ("lr", C.c_float), ("weight_decay", C.c_float),
+                ("beta1", C.c_float), ("beta2", C.c_float), ("eps", C.c_float), ("flags", C.c_int32)]
+
+
 _PROTOTYPES = {
     "sod_version": (C.c_int, []),
     "sod_strerror": (C.c_char_p, [C.c_int]),
@@ -61,6 +68,12 @@ _PROTOTYPES = {
                                    C.POINTER(sod_sgd_segment), C.c_int, C.c_void_p, C.c_float, C.c_void_p, C.c_int, C.c_void_p]),
     "sod_allreduce_sgd": (C.c_int, [C.POINTER(sod_comm), C.c_uint64, C.c_uint64, C.c_uint64, C.c_void_p, C.c_void_p, C.c_int64,
                                     C.POINTER(sod_sgd_segment), C.c_int, C.c_void_p, C.c_float, C.c_void_p, C.c_int, C.c_void_p]),
+    "sod_adam": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
+                           C.POINTER(sod_adam_segment), C.c_int, C.c_void_p, C.c_void_p, C.c_float, C.c_void_p, C.c_int,
+                           C.c_void_p]),
+    "sod_allreduce_adam": (C.c_int, [C.POINTER(sod_comm), C.c_uint64, C.c_uint64, C.c_uint64, C.c_void_p, C.c_void_p,
+                                     C.c_void_p, C.c_int64, C.POINTER(sod_adam_segment), C.c_int, C.c_void_p, C.c_void_p,
+                                     C.c_float, C.c_void_p, C.c_int, C.c_void_p]),
     "sod_grad_gather16": (C.c_int, [C.POINTER(sod_gather_item), C.c_int, C.c_void_p, C.c_int64, C.c_void_p]),
     "sod_grad_merge_bf16": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
     "sod_grad_nonfinite": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),

@@ -15,7 +15,7 @@ import functools
 import torch
 
 from . import _lib
-from .optim import FusedSGD
+from .optim import FusedOptimizer
 
 import os
 
@@ -100,7 +100,7 @@ def initialize(model, optimizer=None, opt_level: str = "O1", dtype: torch.dtype 
                 return inner(*a, **k)
 
         model.forward = autocast_forward
-        if shadow_weights and dtype == torch.bfloat16 and isinstance(optimizer, FusedSGD) and optimizer.flat.param.is_cuda:
+        if shadow_weights and dtype == torch.bfloat16 and isinstance(optimizer, FusedOptimizer) and optimizer.flat.param.is_cuda:
             optimizer.flat.enable_shadow(dtype)
             _install_shadow_weights(model, optimizer.flat)
     return (model, optimizer) if optimizer is not None else model
@@ -112,8 +112,8 @@ def scale_loss(loss, optimizer):
     if not _cfg["dynamic"]:
         yield loss
         return
-    if not isinstance(optimizer, FusedSGD):
-        raise _lib.SodError("fp16 dynamic loss scaling is wired into FusedSGD only")
+    if not isinstance(optimizer, FusedOptimizer):
+        raise _lib.SodError("fp16 dynamic loss scaling is wired into the fused optimizers (FusedSGD, FusedAdam) only")
     scale = _cfg["scale"]
     yield loss * scale
     flat = optimizer.flat

@@ -8,7 +8,8 @@ Layout kept byte-for-byte compatible at the key level:
 `net_state` keys are the un-prefixed module names (the wrapper's `.module` is unwrapped, utils/pipeline_ops.py:68),
 `opti_state` is `torch.optim.SGD`'s state_dict layout (per-parameter `momentum_buffer`) — `FusedSGD.state_dict()`
 materialises it from the flat momentum buffer and `load_state_dict` scatters it back, so checkpoints written by
-the reference load here and vice versa.
+the reference load here and vice versa.  With optim "adam" it is `torch.optim.Adam`'s layout (per-parameter `step`,
+`exp_avg`, `exp_avg_sq`), which `FusedAdam` writes and reads the same way.
 
 One deliberate difference (SURVEY Q5): the reference resumes on rank 0 only, leaving the other ranks at their
 initial weights; here every rank calls `resume_checkpoint` and loads the same file.
@@ -44,8 +45,8 @@ def save_checkpoint(model: nn.Module = None, optimizer: Optimizer = None, amp=No
                     full_net_path: str = "", state_net_path: str = "", write: bool | None = None):
     """Full checkpoint (model + optimizer + amp) and the weights-only file, as the reference writes them.
 
-    Distributed: EVERY rank must call this (the momentum of `FusedSGD` is sharded over the ranks and `state_dict()`
-    gathers it with collectives); only the rank with `write=True` (default: rank 0) touches the files, and all ranks
+    Distributed: EVERY rank must call this (the momentum of `FusedSGD`, and Adam's two moments, are sharded over the
+    ranks and `state_dict()` gathers them with collectives); only the rank with `write=True` (default: rank 0) touches the files, and all ranks
     leave through a barrier so that nobody runs ahead into the next iteration's device-side barriers while rank 0 is
     still writing."""
     import torch.distributed as dist

@@ -1,23 +1,29 @@
-// sgd.cu — gradient all-reduce ⊕ unscale ⊕ SGD-momentum over flat fp32 buffers, plus the plain
-// peer-memory all-reduce used by the bandwidth sweep.
+// sgd.cu — gradient all-reduce ⊕ unscale ⊕ optimizer step (SGD-momentum, optionally Nesterov, or Adam) over flat fp32
+// buffers, plus the plain peer-memory all-reduce used by the bandwidth sweep.
 //
 // Reference arithmetic being replaced (paths relative to the reference repo):
 //   apex DDP(delay_allreduce=True): flat SUM all-reduce then ×1/W            train.py:185
 //   apex amp unscale ×1/S with overflow skip                                  train.py:299
-//   torch.optim.SGD.step (momentum, wd folded into g, no nesterov/dampening)  train.py:303,
-//       groups from make_optimizer("f3_trick")                                utils/pipeline_ops.py:295-313
+//   torch.optim.SGD.step (momentum, wd folded into g, no dampening, nesterov  train.py:303,
+//       per segment) with groups from make_optimizer("f3_trick"/"sgd_trick")  utils/pipeline_ops.py:235-313
+//   torch.optim.Adam.step (L2 weight decay, no amsgrad) of make_optimizer("adam") utils/pipeline_ops.py:287-294
 //   optimizer.zero_grad                                                       train.py:297
 //
-// world == 1 : one streaming pass, 20 B/elem (read g,p,v; write p,v) [+4 B/elem to zero g].
+// world == 1 : one streaming pass, 20 B/elem (read g,p,v; write p,v) [+4 B/elem to zero g]; Adam 28 B/elem (+ m).
 // world  > 1 : two-shot over NVSwitch peer memory. Rank r owns shard r of the flat index space:
 //     start barrier → reduce shard r across ranks (multimem.ld_reduce in the switch, or peer loads
 //     summed in rank order) → unscale/÷W → SGD on (p,v) shard in registers → write the UPDATED
 //     PARAMETERS to every rank (multimem.st / peer stores) → end barrier [→ zero local grads].
 //   So what crosses NVLink is reduce-scatter(grads) + all-gather(params): the same bus bytes as an
 //   all-reduce, but no separate NCCL call, no ÷W pass, no optimizer kernel, and momentum is only ever
-//   touched on the owning rank (1/W of the optimizer-state traffic).
+//   touched on the owning rank (1/W of the optimizer-state traffic; the same holds for Adam's m and v).
+// Both kernels are templates on the update rule (SgdRule / AdamRule below): the segment walk, the bf16-gradient
+// handling, the exchange and the zero-grad / shadow tail exist once.
 //   Owner-computes + broadcast also makes parameters bit-identical on all ranks by construction.
 #include "common.cuh"
+
+#include <cstdio>
+#include <cstdlib>
 
 namespace sod {
 namespace {
@@ -28,21 +34,64 @@ constexpr int kUnroll = 4;
 struct SegTable {
     int n;
     long long begin[SOD_MAX_SEGMENTS], end[SOD_MAX_SEGMENTS];  // in float4 units
-    float lr[SOD_MAX_SEGMENTS], wd[SOD_MAX_SEGMENTS], mu[SOD_MAX_SEGMENTS];
+    float lr[SOD_MAX_SEGMENTS], wd[SOD_MAX_SEGMENTS];
+    float mu[SOD_MAX_SEGMENTS];                              // SGD momentum
+    // Adam: β1, β2 as the decimals the caller wrote (see adam_beta), 1-β1 and 1-β2 rounded to fp32 as torch rounds the
+    // Python scalars, β2 and eps in fp32
+    double beta1d[SOD_MAX_SEGMENTS], beta2d[SOD_MAX_SEGMENTS];
+    float w1[SOD_MAX_SEGMENTS], c2[SOD_MAX_SEGMENTS], beta2[SOD_MAX_SEGMENTS], eps[SOD_MAX_SEGMENTS];
     int flags[SOD_MAX_SEGMENTS];
 };
 
-static int make_seg_table(const sod_sgd_segment* segs, int nseg, int64_t n, SegTable& t) {
+// the range and flag fields shared by both segment kinds
+template <class Seg>
+static int make_seg_ranges(const Seg* segs, int nseg, int64_t n, SegTable& t) {
     if (nseg < 0 || nseg > SOD_MAX_SEGMENTS || (nseg > 0 && segs == nullptr)) return SOD_EINVAL;
     t.n = nseg;
     long long prev = 0;
     for (int i = 0; i < nseg; ++i) {
-        const sod_sgd_segment& s = segs[i];
+        const Seg& s = segs[i];
         if (s.begin < prev || s.end < s.begin || s.end > n) return SOD_EINVAL;  // sorted, disjoint, in range
         if ((s.begin & 3) || (s.end & 3)) return SOD_EALIGN;
         t.begin[i] = s.begin >> 2; t.end[i] = s.end >> 2;
-        t.lr[i] = s.lr; t.wd[i] = s.weight_decay; t.mu[i] = s.momentum; t.flags[i] = s.flags;
+        t.lr[i] = s.lr; t.wd[i] = s.weight_decay; t.flags[i] = s.flags;
+        t.mu[i] = 0.f; t.beta1d[i] = t.beta2d[i] = 0.0; t.w1[i] = t.c2[i] = t.beta2[i] = t.eps[i] = 0.f;
         prev = s.end;
+    }
+    return SOD_OK;
+}
+
+static int make_seg_table(const sod_sgd_segment* segs, int nseg, int64_t n, SegTable& t) {
+    const int rc = make_seg_ranges(segs, nseg, n, t);
+    if (rc != SOD_OK) return rc;
+    for (int i = 0; i < nseg; ++i) t.mu[i] = segs[i].momentum;
+    return SOD_OK;
+}
+
+// The segment carries β as fp32, torch.optim.Adam as a Python float: 0.999f is 0.99900001287…, and 1 - 0.999f differs from
+// fp32(1 - 0.999) by 1.3e-5 relative.  Recover the decimal the caller wrote — the shortest one that rounds to the same
+// fp32 value, which is what an fp32 of a literal like 0.9 or 0.999 came from — so that 1-β and the bias corrections are
+// formed from the same double torch uses.
+static double adam_beta(float b) {
+    char buf[32];
+    for (int digits = 1; digits <= 9; ++digits) {
+        snprintf(buf, sizeof(buf), "%.*g", digits, static_cast<double>(b));
+        const double d = strtod(buf, nullptr);
+        if (static_cast<float>(d) == b) return d;
+    }
+    return static_cast<double>(b);
+}
+
+static int make_seg_table(const sod_adam_segment* segs, int nseg, int64_t n, SegTable& t) {
+    const int rc = make_seg_ranges(segs, nseg, n, t);
+    if (rc != SOD_OK) return rc;
+    for (int i = 0; i < nseg; ++i) {
+        const sod_adam_segment& s = segs[i];
+        if (!(s.beta1 >= 0.f && s.beta1 < 1.f && s.beta2 >= 0.f && s.beta2 < 1.f && s.eps >= 0.f)) return SOD_EINVAL;
+        if (s.flags & SOD_SEG_NESTEROV) return SOD_EINVAL;
+        t.beta1d[i] = adam_beta(s.beta1); t.beta2d[i] = adam_beta(s.beta2);
+        t.w1[i] = static_cast<float>(1.0 - t.beta1d[i]); t.c2[i] = static_cast<float>(1.0 - t.beta2d[i]);
+        t.beta2[i] = s.beta2; t.eps[i] = s.eps;
     }
     return SOD_OK;
 }
@@ -67,12 +116,102 @@ struct SegCursor {
     }
 };
 
-__device__ __forceinline__ void sgd_update(float4& p, float4& v, const float4& g, float lr, float wd, float mu) {
+__device__ __forceinline__ void sgd_update(float4& p, float4& v, const float4& g, float lr, float wd, float mu, bool nesterov) {
     // g' = g + wd*p ; v = mu*v + g' ; p = p - lr*v   (operation order of torch/optim/sgd.py:343-380)
+    // nesterov:                       p = p - lr*(g' + mu*v)
     float gx = fmaf(wd, p.x, g.x), gy = fmaf(wd, p.y, g.y), gz = fmaf(wd, p.z, g.z), gw = fmaf(wd, p.w, g.w);
     v.x = fmaf(mu, v.x, gx); v.y = fmaf(mu, v.y, gy); v.z = fmaf(mu, v.z, gz); v.w = fmaf(mu, v.w, gw);
-    p.x = fmaf(-lr, v.x, p.x); p.y = fmaf(-lr, v.y, p.y); p.z = fmaf(-lr, v.z, p.z); p.w = fmaf(-lr, v.w, p.w);
+    if (nesterov) {
+        gx = fmaf(mu, v.x, gx); gy = fmaf(mu, v.y, gy); gz = fmaf(mu, v.z, gz); gw = fmaf(mu, v.w, gw);
+    } else {
+        gx = v.x; gy = v.y; gz = v.z; gw = v.w;
+    }
+    p.x = fmaf(-lr, gx, p.x); p.y = fmaf(-lr, gy, p.y); p.z = fmaf(-lr, gz, p.z); p.w = fmaf(-lr, gw, p.w);
 }
+
+// An update rule is what the two step kernels below are templated on:
+//   State                per-vector optimizer state held in registers between load and store
+//   Cta                  per-CTA constants, computed once into shared memory by prologue()
+//   load / store         the state of flat vector i
+//   update               one float4 of parameters, given the unscaled-and-averaged gradient and its segment
+//   epilogue             after the last access of the CTA (Adam: the last CTA advances the step counters)
+// kNesterov: some segment carries SOD_SEG_NESTEROV (the plain instantiation is the kernel without that select)
+template <bool kNesterov>
+struct SgdRule {
+    static constexpr bool kHasCta = false;
+    float4* __restrict__ v;
+    struct State { float4 v; };
+    struct Cta {};
+    __device__ __forceinline__ void prologue(Cta&, const SegTable&, const float*) const {}
+    __device__ __forceinline__ void load(State& st, long long i) const { st.v = v[i]; }
+    __device__ __forceinline__ void store(const State& st, long long i) const { v[i] = st.v; }
+    __device__ __forceinline__ void update(float4& p, State& st, const float4& g, const SegTable& segs, const float* lr_dev,
+                                           const Cta&, int s) const {
+        sgd_update(p, st.v, g, seg_lr(segs, lr_dev, s), segs.wd[s], segs.mu[s], kNesterov && (segs.flags[s] & SOD_SEG_NESTEROV));
+    }
+    __device__ __forceinline__ void epilogue(const SegTable&, bool) const {}
+};
+
+__device__ __forceinline__ void adam_update1(float& p, float& m, float& v, float g, float wd, float w1, float b2, float c2,
+                                             float step_size, float bc2_sqrt, float eps) {
+    // torch/optim/adam.py _single_tensor_adam (amsgrad=False, maximize=False, L2 weight decay):
+    //   g' = g + wd*p ; m.lerp_(g', 1-β1) ; v.mul_(β2).addcmul_(g', g', 1-β2) ;
+    //   p.addcdiv_(m, sqrt(v)/bc2_sqrt + eps, -step_size)          IEEE sqrt and division (no fast-math in this build)
+    const float gg = fmaf(wd, p, g);
+    m = fmaf(w1, gg - m, m);
+    v = fmaf(c2 * gg, gg, v * b2);
+    const float denom = sqrtf(v) / bc2_sqrt + eps;
+    p = fmaf(-step_size, m / denom, p);
+}
+
+struct AdamRule {
+    static constexpr bool kHasCta = true;
+    float4* __restrict__ m;
+    float4* __restrict__ v;
+    int32_t* step;          // [SOD_MAX_SEGMENTS] step counts, then the CTA ticket (sod_adam in include/sod_b200.h)
+    struct State { float4 m, v; };
+    struct Cta { float step_size[SOD_MAX_SEGMENTS], bc2_sqrt[SOD_MAX_SEGMENTS]; };
+    // bias corrections of step t = step+1, in fp64 once per CTA and segment, rounded as torch rounds the Python scalars
+    __device__ __forceinline__ void prologue(Cta& cta, const SegTable& segs, const float* lr_dev) const {
+        const int s = threadIdx.x;
+        if (s < segs.n) {
+            const double t = static_cast<double>(step[s]) + 1.0;
+            const double bc1 = 1.0 - pow(segs.beta1d[s], t);
+            const double bc2 = 1.0 - pow(segs.beta2d[s], t);
+            cta.step_size[s] = static_cast<float>(static_cast<double>(seg_lr(segs, lr_dev, s)) / bc1);
+            cta.bc2_sqrt[s] = static_cast<float>(sqrt(bc2));
+        }
+    }
+    __device__ __forceinline__ void load(State& st, long long i) const { st.m = m[i]; st.v = v[i]; }
+    __device__ __forceinline__ void store(const State& st, long long i) const { m[i] = st.m; v[i] = st.v; }
+    __device__ __forceinline__ void update(float4& p, State& st, const float4& g, const SegTable& segs, const float*,
+                                           const Cta& cta, int s) const {
+        const float wd = segs.wd[s], b2 = segs.beta2[s], eps = segs.eps[s], w1 = segs.w1[s], c2 = segs.c2[s];
+        const float ss = cta.step_size[s], bs = cta.bc2_sqrt[s];
+        adam_update1(p.x, st.m.x, st.v.x, g.x, wd, w1, b2, c2, ss, bs, eps);
+        adam_update1(p.y, st.m.y, st.v.y, g.y, wd, w1, b2, c2, ss, bs, eps);
+        adam_update1(p.z, st.m.z, st.v.z, g.z, wd, w1, b2, c2, ss, bs, eps);
+        adam_update1(p.w, st.m.w, st.v.w, g.w, wd, w1, b2, c2, ss, bs, eps);
+    }
+    // every CTA read the counters in its prologue; the last one to get here (ticket, as in resample.cu's colsum) advances
+    // them — unless the step was skipped for an amp overflow — and re-arms the ticket for the next launch
+    __device__ __forceinline__ void epilogue(const SegTable& segs, bool skip) const {
+        __shared__ bool s_last;
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            __threadfence();
+            s_last = atomicAdd(reinterpret_cast<unsigned*>(step + SOD_MAX_SEGMENTS), 1u) == gridDim.x - 1;
+        }
+        __syncthreads();
+        if (s_last && threadIdx.x == 0) {
+            __threadfence();
+            if (!skip)
+                for (int s = 0; s < segs.n; ++s)
+                    if (!(segs.flags[s] & SOD_SEG_FROZEN)) step[s] += 1;
+            step[SOD_MAX_SEGMENTS] = 0;
+        }
+    }
+};
 
 // ------------------------------------------------------------------------------------------------
 // world == 1
@@ -90,18 +229,23 @@ __device__ __forceinline__ uint2 f32x4_to_bf16(const float4& f) {
     return u;
 }
 
-__global__ void __launch_bounds__(kThreads) sgd_local_kernel(float4* __restrict__ p, float4* __restrict__ v,
-                                                             float4* __restrict__ g, uint2* __restrict__ g16,
-                                                             uint2* __restrict__ shadow, long long nvec,
-                                                             const __grid_constant__ SegTable segs, float inv_scale,
-                                                             const uint32_t* found_inf, int zero_grad,
-                                                             const float* __restrict__ lr_dev) {
+template <class Rule>
+__global__ void __launch_bounds__(kThreads) local_step_kernel(float4* __restrict__ p, const Rule rule,
+                                                              float4* __restrict__ g, uint2* __restrict__ g16,
+                                                              uint2* __restrict__ shadow, long long nvec,
+                                                              const __grid_constant__ SegTable segs, float inv_scale,
+                                                              const uint32_t* found_inf, int zero_grad,
+                                                              const float* __restrict__ lr_dev) {
     const bool skip = (found_inf != nullptr && *found_inf != 0);  // amp overflow: no update, but still clear g
+    __shared__ typename Rule::Cta cta;
+    rule.prologue(cta, segs, lr_dev);
+    if constexpr (Rule::kHasCta) __syncthreads();
     SegCursor cur;
     const long long stride = static_cast<long long>(gridDim.x) * kThreads;
     const float4 zero = make_float4(0.f, 0.f, 0.f, 0.f);
     for (long long i0 = static_cast<long long>(blockIdx.x) * kThreads + threadIdx.x; i0 < nvec; i0 += stride * kUnroll) {
-        float4 gv[kUnroll], pv[kUnroll], vv[kUnroll];
+        float4 gv[kUnroll], pv[kUnroll];
+        typename Rule::State st[kUnroll];
         int sidx[kUnroll];
         bool only16[kUnroll];
 #pragma unroll
@@ -125,7 +269,7 @@ __global__ void __launch_bounds__(kThreads) sgd_local_kernel(float4* __restrict_
                 if (!skip && in_seg && !(segs.flags[cur.s] & SOD_SEG_FROZEN)) {
                     sidx[u] = cur.s;
                     pv[u] = p[i];
-                    vv[u] = v[i];
+                    rule.load(st[u], i);
                 }
             }
         }
@@ -136,9 +280,9 @@ __global__ void __launch_bounds__(kThreads) sgd_local_kernel(float4* __restrict_
                 if (sidx[u] >= 0) {
                     const int s = sidx[u];
                     const float4 gs = make_float4(gv[u].x * inv_scale, gv[u].y * inv_scale, gv[u].z * inv_scale, gv[u].w * inv_scale);
-                    sgd_update(pv[u], vv[u], gs, seg_lr(segs, lr_dev, s), segs.wd[s], segs.mu[s]);
+                    rule.update(pv[u], st[u], gs, segs, lr_dev, cta, s);
                     p[i] = pv[u];
-                    v[i] = vv[u];
+                    rule.store(st[u], i);
                     if (shadow != nullptr) shadow[i] = f32x4_to_bf16(pv[u]);
                 }
                 if (zero_grad) {
@@ -148,6 +292,7 @@ __global__ void __launch_bounds__(kThreads) sgd_local_kernel(float4* __restrict_
             }
         }
     }
+    rule.epilogue(segs, skip);
 }
 
 __global__ void grad_merge_bf16_kernel(float4* __restrict__ g, uint2* __restrict__ g16, long long nvec) {
@@ -255,15 +400,17 @@ __device__ __forceinline__ float4 reduce_vec16(const CommDev& c, uint64_t byte_o
     return acc;
 }
 
-template <bool kMulticast>
-__global__ void __launch_bounds__(kThreads) allreduce_sgd_kernel(const __grid_constant__ CommDev c, uint64_t grad_off,
-                                                                 uint64_t param_off, float4* __restrict__ mom,
-                                                                 long long nvec, const __grid_constant__ SegTable segs,
-                                                                 float scale, const uint32_t* found_inf,
-                                                                 int zero_grad, uint2* __restrict__ shadow,
-                                                                 const float* __restrict__ lr_dev, uint64_t grad16_off,
-                                                                 int has_grad16) {
+template <class Rule, bool kMulticast>
+__global__ void __launch_bounds__(kThreads) allreduce_step_kernel(const __grid_constant__ CommDev c, uint64_t grad_off,
+                                                                  uint64_t param_off, const Rule rule,
+                                                                  long long nvec, const __grid_constant__ SegTable segs,
+                                                                  float scale, const uint32_t* found_inf,
+                                                                  int zero_grad, uint2* __restrict__ shadow,
+                                                                  const float* __restrict__ lr_dev, uint64_t grad16_off,
+                                                                  int has_grad16) {
     const bool skip = (found_inf != nullptr && *found_inf != 0);  // caller guarantees identical on all ranks
+    __shared__ typename Rule::Cta cta;
+    rule.prologue(cta, segs, lr_dev);                             // (the barrier below orders it for the whole CTA)
     // every rank's backward has finished writing its gradients
     if (!comm_block_barrier(c, 0, blockIdx.x)) return;
 
@@ -295,10 +442,12 @@ __global__ void __launch_bounds__(kThreads) allreduce_sgd_kernel(const __grid_co
                 const long long i = i0 + u * stride;
                 if (sidx[u] >= 0) {
                     const int s = sidx[u];
-                    float4 pv = p_local[i], vv = mom[i];
+                    float4 pv = p_local[i];
+                    typename Rule::State st;
+                    rule.load(st, i);
                     const float4 gs = make_float4(gv[u].x * scale, gv[u].y * scale, gv[u].z * scale, gv[u].w * scale);
-                    sgd_update(pv, vv, gs, seg_lr(segs, lr_dev, s), segs.wd[s], segs.mu[s]);
-                    mom[i] = vv;
+                    rule.update(pv, st, gs, segs, lr_dev, cta, s);
+                    rule.store(st, i);
                     broadcast_vec<kMulticast>(c, param_off + static_cast<uint64_t>(i) * 16u, pv);
                 }
             }
@@ -329,6 +478,7 @@ __global__ void __launch_bounds__(kThreads) allreduce_sgd_kernel(const __grid_co
             }
         }
     }
+    rule.epilogue(segs, skip);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -398,12 +548,21 @@ static unsigned comm_grid(long long vecs_per_rank) {
 }  // namespace
 }  // namespace sod
 
-extern "C" int sod_sgd_momentum(float* param, float* mom, float* grad, void* grad16, void* shadow16, int64_t n,
-                                const sod_sgd_segment* segs, int nseg, const float* lr_dev, float inv_scale,
-                                const uint32_t* found_inf, int flags, void* stream) {
-    using namespace sod;
-    SOD_CHECK_ARG(param && mom && grad && n > 0, SOD_EINVAL);
-    SOD_CHECK_ARG((n & 3) == 0 && aligned16(param) && aligned16(mom) && aligned16(grad), SOD_EALIGN);
+namespace sod {
+namespace {
+
+static bool any_nesterov(const sod_sgd_segment* segs, int nseg) {
+    for (int i = 0; segs != nullptr && i < nseg && i < SOD_MAX_SEGMENTS; ++i)
+        if (segs[i].flags & SOD_SEG_NESTEROV) return true;
+    return false;
+}
+
+// world 1: validation shared by sod_sgd_momentum and sod_adam, then one streaming launch of local_step_kernel<Rule>
+template <class Rule, class Seg>
+int launch_local_step(float* param, const Rule& rule, float* grad, void* grad16, void* shadow16, int64_t n, const Seg* segs,
+                      int nseg, const float* lr_dev, float inv_scale, const uint32_t* found_inf, int flags, void* stream) {
+    SOD_CHECK_ARG(param && grad && n > 0, SOD_EINVAL);
+    SOD_CHECK_ARG((n & 3) == 0 && aligned16(param) && aligned16(grad), SOD_EALIGN);
     SOD_CHECK_ARG((!grad16 || aligned16(grad16)) && (!shadow16 || aligned16(shadow16)), SOD_EALIGN);
     SegTable t;
     int rc = make_seg_table(segs, nseg, n, t);
@@ -412,11 +571,75 @@ extern "C" int sod_sgd_momentum(float* param, float* mom, float* grad, void* gra
     long long blocks = (nvec + static_cast<long long>(kThreads) * kUnroll - 1) / (static_cast<long long>(kThreads) * kUnroll);
     const long long cap = 2ll * dev_info().sm_count;
     if (blocks > cap) blocks = cap;
-    sgd_local_kernel<<<static_cast<unsigned>(blocks), kThreads, 0, static_cast<cudaStream_t>(stream)>>>(
-        reinterpret_cast<float4*>(param), reinterpret_cast<float4*>(mom), reinterpret_cast<float4*>(grad),
+    local_step_kernel<Rule><<<static_cast<unsigned>(blocks), kThreads, 0, static_cast<cudaStream_t>(stream)>>>(
+        reinterpret_cast<float4*>(param), rule, reinterpret_cast<float4*>(grad),
         reinterpret_cast<uint2*>(grad16), reinterpret_cast<uint2*>(shadow16), nvec, t, inv_scale, found_inf,
         (flags & SOD_SGD_ZERO_GRAD) ? 1 : 0, lr_dev);
     return static_cast<int>(cudaGetLastError());
+}
+
+// world > 1: validation shared by sod_allreduce_sgd and sod_allreduce_adam, then allreduce_step_kernel<Rule, multicast?>
+template <class Rule, class Seg>
+int launch_allreduce_step(const sod_comm* comm, uint64_t grad_off, uint64_t grad16_off, uint64_t param_off, const Rule& rule,
+                          void* shadow16, int64_t n, const Seg* segs, int nseg, const float* lr_dev, float inv_scale,
+                          const uint32_t* found_inf, int flags, void* stream) {
+    SOD_CHECK_ARG(comm && n > 0, SOD_EINVAL);
+    SOD_CHECK_ARG((n & 3) == 0 && (grad_off & 15) == 0 && (param_off & 15) == 0, SOD_EALIGN);
+    CommDev c;
+    int rc = make_comm_dev(comm, c);
+    if (rc != SOD_OK) return rc;
+    SOD_CHECK_ARG(grad_off >= sod_comm_flag_bytes() && param_off >= sod_comm_flag_bytes(), SOD_ECOMM);
+    SOD_CHECK_ARG(grad_off + static_cast<uint64_t>(n) * 4 <= comm->arena_bytes &&
+                      param_off + static_cast<uint64_t>(n) * 4 <= comm->arena_bytes, SOD_ECOMM);
+    const int has16 = grad16_off != 0 ? 1 : 0;
+    if (has16) {
+        SOD_CHECK_ARG((grad16_off & 15) == 0, SOD_EALIGN);
+        SOD_CHECK_ARG(grad16_off >= sod_comm_flag_bytes() && grad16_off + static_cast<uint64_t>(n) * 2 <= comm->arena_bytes, SOD_ECOMM);
+    }
+    SegTable t;
+    rc = make_seg_table(segs, nseg, n, t);
+    if (rc != SOD_OK) return rc;
+    const long long nvec = n >> 2;
+    const unsigned grid = comm_grid((nvec + c.world - 1) / c.world);
+    const float scale = inv_scale / static_cast<float>(c.world);
+    const int zg = (flags & SOD_SGD_ZERO_GRAD) ? 1 : 0;
+    // with two ranks plain peer loads move the gradient bucket faster than the in-switch reduction; from four ranks up
+    // NVLS wins (an all-reduce sweep, `bench.py --sweep`, decides this per system)
+    const bool mc = (c.mc != 0) && !(flags & SOD_ALGO_NO_MULTIMEM) && (c.world > 2 || (flags & SOD_ALGO_FORCE_MULTIMEM));
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    if (mc)
+        allreduce_step_kernel<Rule, true><<<grid, kThreads, 0, s>>>(c, grad_off, param_off, rule, nvec, t, scale, found_inf, zg,
+                                                                    reinterpret_cast<uint2*>(shadow16), lr_dev, grad16_off, has16);
+    else
+        allreduce_step_kernel<Rule, false><<<grid, kThreads, 0, s>>>(c, grad_off, param_off, rule, nvec, t, scale, found_inf, zg,
+                                                                     reinterpret_cast<uint2*>(shadow16), lr_dev, grad16_off, has16);
+    return static_cast<int>(cudaGetLastError());
+}
+
+}  // namespace
+}  // namespace sod
+
+extern "C" int sod_sgd_momentum(float* param, float* mom, float* grad, void* grad16, void* shadow16, int64_t n,
+                                const sod_sgd_segment* segs, int nseg, const float* lr_dev, float inv_scale,
+                                const uint32_t* found_inf, int flags, void* stream) {
+    using namespace sod;
+    SOD_CHECK_ARG(param && mom && grad && n > 0, SOD_EINVAL);
+    SOD_CHECK_ARG(aligned16(mom), SOD_EALIGN);
+    if (any_nesterov(segs, nseg))
+        return launch_local_step(param, SgdRule<true>{reinterpret_cast<float4*>(mom)}, grad, grad16, shadow16, n, segs, nseg,
+                                 lr_dev, inv_scale, found_inf, flags, stream);
+    return launch_local_step(param, SgdRule<false>{reinterpret_cast<float4*>(mom)}, grad, grad16, shadow16, n, segs, nseg,
+                             lr_dev, inv_scale, found_inf, flags, stream);
+}
+
+extern "C" int sod_adam(float* param, float* exp_avg, float* exp_avg_sq, float* grad, void* grad16, void* shadow16, int64_t n,
+                        const sod_adam_segment* segs, int nseg, const float* lr_dev, int32_t* step_dev, float inv_scale,
+                        const uint32_t* found_inf, int flags, void* stream) {
+    using namespace sod;
+    SOD_CHECK_ARG(param && exp_avg && exp_avg_sq && step_dev && grad && n > 0, SOD_EINVAL);
+    SOD_CHECK_ARG(aligned16(exp_avg) && aligned16(exp_avg_sq), SOD_EALIGN);
+    const AdamRule rule{reinterpret_cast<float4*>(exp_avg), reinterpret_cast<float4*>(exp_avg_sq), step_dev};
+    return launch_local_step(param, rule, grad, grad16, shadow16, n, segs, nseg, lr_dev, inv_scale, found_inf, flags, stream);
 }
 
 extern "C" int sod_grad_gather16(const sod_gather_item* items, int nitems, void* dst16, int64_t dst_elems, void* stream) {
@@ -480,36 +703,24 @@ extern "C" int sod_allreduce_sgd(const sod_comm* comm, uint64_t grad_off, uint64
                                  float inv_scale, const uint32_t* found_inf, int flags, void* stream) {
     using namespace sod;
     SOD_CHECK_ARG(comm && mom && n > 0, SOD_EINVAL);
-    SOD_CHECK_ARG((n & 3) == 0 && aligned16(mom) && (grad_off & 15) == 0 && (param_off & 15) == 0, SOD_EALIGN);
-    CommDev c;
-    int rc = make_comm_dev(comm, c);
-    if (rc != SOD_OK) return rc;
-    SOD_CHECK_ARG(grad_off >= sod_comm_flag_bytes() && param_off >= sod_comm_flag_bytes(), SOD_ECOMM);
-    SOD_CHECK_ARG(grad_off + static_cast<uint64_t>(n) * 4 <= comm->arena_bytes &&
-                      param_off + static_cast<uint64_t>(n) * 4 <= comm->arena_bytes, SOD_ECOMM);
-    const int has16 = grad16_off != 0 ? 1 : 0;
-    if (has16) {
-        SOD_CHECK_ARG((grad16_off & 15) == 0, SOD_EALIGN);
-        SOD_CHECK_ARG(grad16_off >= sod_comm_flag_bytes() && grad16_off + static_cast<uint64_t>(n) * 2 <= comm->arena_bytes, SOD_ECOMM);
-    }
-    SegTable t;
-    rc = make_seg_table(segs, nseg, n, t);
-    if (rc != SOD_OK) return rc;
-    const long long nvec = n >> 2;
-    const unsigned grid = comm_grid((nvec + c.world - 1) / c.world);
-    const float scale = inv_scale / static_cast<float>(c.world);
-    const int zg = (flags & SOD_SGD_ZERO_GRAD) ? 1 : 0;
-    // with two ranks plain peer loads move the gradient bucket faster than the in-switch reduction; from four ranks up
-    // NVLS wins (an all-reduce sweep, `bench.py --sweep`, decides this per system)
-    const bool mc = (c.mc != 0) && !(flags & SOD_ALGO_NO_MULTIMEM) && (c.world > 2 || (flags & SOD_ALGO_FORCE_MULTIMEM));
-    cudaStream_t s = static_cast<cudaStream_t>(stream);
-    if (mc)
-        allreduce_sgd_kernel<true><<<grid, kThreads, 0, s>>>(c, grad_off, param_off, reinterpret_cast<float4*>(mom), nvec, t,
-                                                             scale, found_inf, zg, reinterpret_cast<uint2*>(shadow16), lr_dev, grad16_off, has16);
-    else
-        allreduce_sgd_kernel<false><<<grid, kThreads, 0, s>>>(c, grad_off, param_off, reinterpret_cast<float4*>(mom), nvec, t,
-                                                              scale, found_inf, zg, reinterpret_cast<uint2*>(shadow16), lr_dev, grad16_off, has16);
-    return static_cast<int>(cudaGetLastError());
+    SOD_CHECK_ARG(aligned16(mom), SOD_EALIGN);
+    if (any_nesterov(segs, nseg))
+        return launch_allreduce_step(comm, grad_off, grad16_off, param_off, SgdRule<true>{reinterpret_cast<float4*>(mom)},
+                                     shadow16, n, segs, nseg, lr_dev, inv_scale, found_inf, flags, stream);
+    return launch_allreduce_step(comm, grad_off, grad16_off, param_off, SgdRule<false>{reinterpret_cast<float4*>(mom)},
+                                 shadow16, n, segs, nseg, lr_dev, inv_scale, found_inf, flags, stream);
+}
+
+extern "C" int sod_allreduce_adam(const sod_comm* comm, uint64_t grad_off, uint64_t grad16_off, uint64_t param_off,
+                                  float* exp_avg, float* exp_avg_sq, void* shadow16, int64_t n, const sod_adam_segment* segs,
+                                  int nseg, const float* lr_dev, int32_t* step_dev, float inv_scale,
+                                  const uint32_t* found_inf, int flags, void* stream) {
+    using namespace sod;
+    SOD_CHECK_ARG(comm && exp_avg && exp_avg_sq && step_dev && n > 0, SOD_EINVAL);
+    SOD_CHECK_ARG(aligned16(exp_avg) && aligned16(exp_avg_sq), SOD_EALIGN);
+    const AdamRule rule{reinterpret_cast<float4*>(exp_avg), reinterpret_cast<float4*>(exp_avg_sq), step_dev};
+    return launch_allreduce_step(comm, grad_off, grad16_off, param_off, rule, shadow16, n, segs, nseg, lr_dev, inv_scale,
+                                 found_inf, flags, stream);
 }
 
 extern "C" int sod_allreduce_f32(const sod_comm* comm, uint64_t off, int64_t n, float scale, int algo, int flags,

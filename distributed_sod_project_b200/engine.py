@@ -61,9 +61,9 @@ class Trainer:
         self._loss_event: torch.cuda.Event | None = None
         # CUDA-graph replay of the whole iteration (SURVEY §8f.1): one cudaGraphLaunch instead of ~1500 launches.
         # One graph per input shape (multi-scale training, reference utils/dataset.py:125-132, cycles through three);
-        # learning rates are read from a device table (FusedSGD.sync_lr), so the scheduler never forces a re-capture.
-        from .optim import FusedSGD
-        self.use_graph = use_graph and not amp._cfg["dynamic"] and isinstance(self.optimizer, FusedSGD)
+        # learning rates are read from a device table (FusedOptimizer.sync_lr), so the scheduler never forces a re-capture.
+        from .optim import FusedOptimizer
+        self.use_graph = use_graph and not amp._cfg["dynamic"] and isinstance(self.optimizer, FusedOptimizer)
         self._graphs: dict = {}
         self._cur = None
 
@@ -106,22 +106,18 @@ class Trainer:
         """warm up eagerly on a side stream, then record one whole iteration into a CUDA graph"""
         static_x, static_m = x.clone(), m.clone()
         # the warm-up iterations (allocator, cuDNN autotune, autograd thread) must not move the training state
-        flat = self.optimizer.flat
-        snap = [flat.param.clone(), flat.mom.clone()] + [b.clone() for b in self.module.buffers()]
-        shadow_snap = flat.shadow16.clone() if flat.shadow16 is not None else None
-        steps, stepped = self.optimizer.steps, self.optimizer._stepped
+        snap = self.optimizer.snapshot()             # parameters, optimizer state (Adam: its step counts), shadow
+        buffers = [b.clone() for b in self.module.buffers()]
         side = torch.cuda.Stream()
         side.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(side):
             for _ in range(2):
                 self._iteration(static_x, static_m, report=False)
         torch.cuda.current_stream().wait_stream(side)
+        self.optimizer.restore(snap)
         with torch.no_grad():
-            flat.param.copy_(snap[0]); flat.mom.copy_(snap[1])
-            for b, old in zip(self.module.buffers(), snap[2:]):
+            for b, old in zip(self.module.buffers(), buffers):
                 b.copy_(old)
-            if shadow_snap is not None:
-                flat.shadow16.copy_(shadow_snap)
         if self.world > 1:
             torch.distributed.barrier()
         torch.cuda.synchronize()
@@ -135,7 +131,7 @@ class Trainer:
         finally:
             syncbn.begin_iteration(self.device, graph=False)
         # capturing records, it does not execute: the optimizer has not stepped
-        self.optimizer.steps, self.optimizer._stepped = steps, stepped
+        self.optimizer.steps, self.optimizer._stepped = snap["steps"], snap["stepped"]
         return dict(graph=graph, x=static_x, m=static_m, out=(red, items, preds), launches=_lib.launches - launches0)
 
     def _graph_for(self, x: torch.Tensor, m: torch.Tensor) -> dict:

@@ -1,26 +1,28 @@
-"""Optimizer seam: `make_optimizer`, `CustomScheduler`, and `FusedSGD` (csrc/sgd.cu underneath).
+"""Optimizer seam: `make_optimizer`, `CustomScheduler`, `FusedSGD` and `FusedAdam` (csrc/sgd.cu underneath).
 
 Reference surface kept (paths in the reference repo):
 * `make_optimizer(model, optimizer_type, optimizer_info)`          — utils/pipeline_ops.py:235-316
-  (`sgd_trick`, `sgd_r3`, `sgd_all`, `f3_trick` → FusedSGD; `adam` → torch.optim.Adam, not on the hot path)
+  (`sgd_trick`, `sgd_r3`, `sgd_all`, `f3_trick` → FusedSGD, `nesterov` honoured for sgd_trick / f3_trick;
+  `adam` → FusedAdam)
 * `CustomScheduler(optimizer, total_num, scheduler_type, scheduler_info).step(optimizer, curr_epoch)`
                                                                      — utils/pipeline_ops.py:185-232
 * the `torch.optim.Optimizer` protocol the loop relies on: `.param_groups[i]["lr"]` mutated from outside,
-  `.zero_grad()`, `.step()`, `.state_dict()/.load_state_dict()` with per-parameter `momentum_buffer`
-  (utils/pipeline_ops.py:73,118), `str(optimizer)` (train.py:176).
+  `.zero_grad()`, `.step()`, `.state_dict()/.load_state_dict()` with per-parameter `momentum_buffer` (SGD) or
+  `step` / `exp_avg` / `exp_avg_sq` (Adam) (utils/pipeline_ops.py:73,118), `str(optimizer)` (train.py:176).
 
-FusedSGD keeps parameters, gradients and momentum in three flat fp32 buffers laid out group-major
-([group 0 | group 1 | … | parameters in no group]); every `p.data` / `p.grad` is a view into them.  `step()`
-is one kernel: world 1 → `sod_sgd_momentum`; world > 1 (after `DistributedDataParallel` has moved the flat
-parameter and gradient buffers into symmetric memory) → `sod_allreduce_sgd`, which also does the
-gradient averaging, so nothing else runs between backward and the next forward.
+The fused optimizers (`FusedOptimizer` and its two subclasses) keep parameters, gradients and optimizer state in flat
+fp32 buffers laid out group-major ([group 0 | group 1 | … | parameters in no group]); every `p.data` / `p.grad` is a
+view into them.  `step()` is one kernel: world 1 → `sod_sgd_momentum` / `sod_adam`; world > 1 (after
+`DistributedDataParallel` has moved the flat parameter and gradient buffers into symmetric memory) →
+`sod_allreduce_sgd` / `sod_allreduce_adam`, which also do the gradient averaging, so nothing else runs between
+backward and the next forward.
 """
 from __future__ import annotations
 
 import numpy as np
 import torch
 import torch.nn as nn
-from torch.optim import Adam, Optimizer
+from torch.optim import Optimizer
 
 from . import _lib
 
@@ -46,7 +48,7 @@ class FlatParams:
             raise ValueError("no parameters")
         dev = all_params[0].device
         if any(p.device != dev or p.dtype != torch.float32 for p in all_params):
-            raise _lib.SodError("FusedSGD needs fp32 parameters on one device")
+            raise _lib.SodError("the fused optimizers need fp32 parameters on one device")
         self.device = dev
         self.slots: list[tuple[nn.Parameter, int]] = []      # (param, element offset)
         self.ranges: list[tuple[int, int]] = []               # per group [begin, end), then leftovers
@@ -71,7 +73,7 @@ class FlatParams:
         self.grad16: torch.Tensor | None = None     # bf16 gradients autograd accumulates for the shadowed tensors
         # bf16 shadow leaves the convolutions consume (amp._install_shadow_weights): (leaf, element offset, steal)
         # steal=True: `.grad` is left None so that autograd hands over cuDNN's gradient tensor as it is (no accumulate
-        # kernel per parameter); FusedSGD.step collects all of them into `grad16` with one sod_grad_gather16 launch
+        # kernel per parameter); the fused step collects all of them into `grad16` with one sod_grad_gather16 launch
         self.shadow_leaves: list[tuple[torch.Tensor, int, bool]] = []
         # set by a hook on the fp32 masters of shadowed parameters (amp._install_shadow_weights) when a gradient reaches one
         # of them — the model ran outside autocast — and cleared by the step that has consumed it
@@ -164,14 +166,13 @@ def _same_physical_order(a: torch.Tensor, b: torch.Tensor) -> bool:
     return True
 
 
-class FusedSGD(Optimizer):
-    """SGD with momentum / weight decay as one flat sm_90a kernel; gradient averaging folded in when
-    distributed.  Arithmetic = torch.optim.SGD (torch/optim/sgd.py:343-380) with dampening 0, nesterov False."""
+class FusedOptimizer(Optimizer):
+    """What the fused optimizers share: the flat group-major layout (`FlatParams`), the segment table the kernels walk,
+    the device learning-rate table, the bf16 gradient gather, `zero_grad`, the shard bounds of world > 1 and the
+    collective gather of sharded state.  A subclass names its state buffers and its kernels (`_segment`, `_launch_local`,
+    `_launch_allreduce`) and keeps its own torch.optim state_dict layout."""
 
-    def __init__(self, params, lr=1e-3, momentum=0.0, weight_decay=0.0, nesterov=False, model: nn.Module | None = None):
-        if nesterov:
-            raise _lib.SodError("nesterov momentum is not on the reference's hot path (config.py:65 nesterov=False)")
-        defaults = dict(lr=lr, momentum=momentum, weight_decay=weight_decay, nesterov=False, dampening=0)
+    def __init__(self, params, defaults: dict, model: nn.Module | None):
         super().__init__(params, defaults)
         if 2 * (len(self.param_groups) + 1) > _lib.SOD_MAX_SEGMENTS:
             raise _lib.SodError(f"at most {_lib.SOD_MAX_SEGMENTS // 2 - 1} parameter groups")
@@ -194,6 +195,22 @@ class FusedSGD(Optimizer):
             if self.flat.device.type == "cuda" else None
         self._lr_sent: list[float | None] = [None] * _lib.SOD_MAX_SEGMENTS
 
+    # -- what a subclass provides ---------------------------------------------------------------------------
+    def _state_buffers(self) -> list[torch.Tensor]:
+        """the flat optimizer-state buffers (full length; at world > 1 each rank keeps only its shard current)"""
+        raise NotImplementedError
+
+    def _segment(self, b: int, e: int, g: dict | None, flags: int):
+        """one entry of the kernels' segment table; g is None for the frozen parameters outside every group"""
+        raise NotImplementedError
+
+    def _launch_local(self, segs, n, lr_dev, g16, s16, finf) -> None:
+        raise NotImplementedError
+
+    def _launch_allreduce(self, segs, n, lr_dev, g16, s16, finf) -> None:
+        raise NotImplementedError
+
+    # -------------------------------------------------------------------------------------------------------
     def _grad_versions(self):
         f = self.flat
         return (f.grad._version, f.grad16._version if f.grad16 is not None else -1, id(f.grad), _lib.grad_writes)
@@ -230,6 +247,15 @@ class FusedSGD(Optimizer):
             else:
                 plan.append((b, e, g, self.flat.grad16 is not None and mid == e))
         return plan
+
+    def _group_segments(self) -> list[list[int]]:
+        """per param_group, the indices of its segments in `_segment_plan()`"""
+        out: list[list[int]] = [[] for _ in self.param_groups]
+        ids = [id(g) for g in self.param_groups]
+        for n, (_, _, g, _) in enumerate(self._segment_plan()):
+            if g is not None:
+                out[ids.index(id(g))].append(n)
+        return out
 
     # -- torch.optim.Optimizer protocol -------------------------------------------------------------------
     def zero_grad(self, set_to_none: bool = False):
@@ -281,14 +307,11 @@ class FusedSGD(Optimizer):
     def _segments(self):
         plan = self._segment_plan()
         exclusive = self._bf16_exclusive()
-        segs = (_lib.sod_sgd_segment * max(len(plan), 1))()
-        for n, (b, e, g, bf16_part) in enumerate(plan):
+        entries = []
+        for b, e, g, bf16_part in plan:
             flags = _lib.SOD_SEG_GRAD16 if (bf16_part and exclusive) else 0
-            if g is None:
-                segs[n] = _lib.sod_sgd_segment(b, e, 0.0, 0.0, 0.0, flags | _lib.SOD_SEG_FROZEN)
-            else:
-                segs[n] = _lib.sod_sgd_segment(b, e, float(g["lr"]), float(g["weight_decay"]), float(g["momentum"]), flags)
-        return segs, len(plan)
+            entries.append(self._segment(b, e, g, flags | _lib.SOD_SEG_FROZEN if g is None else flags))
+        return (type(entries[0]) * len(entries))(*entries), len(plan)
 
     @torch.no_grad()
     def step(self, closure=None):
@@ -296,7 +319,7 @@ class FusedSGD(Optimizer):
             raise _lib.SodError("closures are not supported by the fused step")
         f = self.flat
         if not f.param.is_cuda:
-            raise _lib.SodError("FusedSGD.step needs CUDA parameters (no CPU fallback)")
+            raise _lib.SodError(f"{type(self).__name__}.step needs CUDA parameters (no CPU fallback)")
         segs, n = self._segments()
         self.sync_lr()
         lr_dev = self._lr_dev.data_ptr()
@@ -305,22 +328,15 @@ class FusedSGD(Optimizer):
         g16 = f.grad16.data_ptr() if f.grad16 is not None else None
         s16 = f.shadow16.data_ptr() if f.shadow16 is not None else None
         if f.arena is None:
-            rc = _lib.lib().sod_sgd_momentum(f.param.data_ptr(), f.mom.data_ptr(), f.grad.data_ptr(), g16, s16, f.numel,
-                                             segs, n, lr_dev, float(self.inv_scale), finf, _lib.SOD_SGD_ZERO_GRAD,
-                                             _lib.stream_ptr())
-            _lib.check(rc, "sod_sgd_momentum")
+            self._launch_local(segs, n, lr_dev, g16, s16, finf)
         else:
-            a = f.arena
             if g16 is not None and not self._bf16_exclusive():
                 # fp32 gradients were written for the convolution parameters too (model ran outside autocast): fold the
                 # bf16 ones into the fp32 symmetric buffer and exchange that
                 rc = _lib.lib().sod_grad_merge_bf16(f.grad.data_ptr(), g16, f.numel, _lib.stream_ptr())
                 _lib.check(rc, "sod_grad_merge_bf16")
                 _lib.count_launch()
-            rc = _lib.lib().sod_allreduce_sgd(a.ref, f.grad_off, f.grad16_off if g16 is not None else 0, f.param_off,
-                                              f.mom.data_ptr(), s16, f.numel, segs, n, lr_dev, float(self.inv_scale), finf,
-                                              _lib.SOD_SGD_ZERO_GRAD, _lib.stream_ptr())
-            _lib.check(rc, "sod_allreduce_sgd")
+            self._launch_allreduce(segs, n, lr_dev, g16, s16, finf)
         _lib.count_launch()
         f.master_grads_seen = False
         self._grads_clean = True
@@ -329,15 +345,16 @@ class FusedSGD(Optimizer):
         self.steps += 1
 
     def shard_bounds(self, rank: int, world: int) -> tuple[int, int]:
-        """element range of the flat buffers rank `rank` owns in `sod_allreduce_sgd` (csrc/sgd.cu: ceil(nvec/W) float4s)"""
+        """element range of the flat buffers rank `rank` owns in the world > 1 step kernels (csrc/sgd.cu: ceil(nvec/W)
+        float4s)"""
         nvec = self.flat.numel // 4
         shard = (nvec + world - 1) // world
         return min(rank * shard, nvec) * 4, min((rank + 1) * shard, nvec) * 4
 
     @torch.no_grad()
-    def gather_momentum(self) -> None:
-        """world > 1: every rank only ever updates the momentum of the shard it owns (ZeRO-1 style); bring the full
-        buffer up to date on every rank.  COLLECTIVE (torch.distributed broadcasts, not on the hot path) — called by
+    def gather_state(self) -> None:
+        """world > 1: every rank only ever updates the optimizer state of the shard it owns (ZeRO-1 style); bring the
+        full buffers up to date on every rank.  COLLECTIVE (torch.distributed broadcasts, not on the hot path) — called by
         `state_dict()`, so `state_dict()` must be entered by all ranks, like the reference's DDP/amp save path runs on
         every process before rank 0 writes the file (utils/pipeline_ops.py:46-78)."""
         f = self.flat
@@ -345,14 +362,69 @@ class FusedSGD(Optimizer):
             return
         import torch.distributed as dist
         world = f.arena.world
-        for r in range(world):
-            lo, hi = self.shard_bounds(r, world)
-            if hi > lo:
-                dist.broadcast(f.mom[lo:hi], src=dist.get_global_rank(f.arena.group, r), group=f.arena.group)
+        for buf in self._state_buffers():
+            for r in range(world):
+                lo, hi = self.shard_bounds(r, world)
+                if hi > lo:
+                    dist.broadcast(buf[lo:hi], src=dist.get_global_rank(f.arena.group, r), group=f.arena.group)
+
+    # -- CUDA-graph capture: the warm-up iterations must not move the training state ------------------------
+    def snapshot(self) -> dict:
+        """copies of everything a step changes: parameters, optimizer state, the bf16 shadow, the step counts"""
+        return dict(tensors=[t.clone() for t in self._snapshot_tensors()], steps=self.steps, stepped=self._stepped)
+
+    @torch.no_grad()
+    def restore(self, snap: dict) -> None:
+        for t, old in zip(self._snapshot_tensors(), snap["tensors"]):
+            t.copy_(old)
+        self.steps, self._stepped = snap["steps"], snap["stepped"]
+
+    def _snapshot_tensors(self) -> list[torch.Tensor]:
+        f = self.flat
+        return [f.param, *self._state_buffers()] + ([f.shadow16] if f.shadow16 is not None else [])
+
+
+class FusedSGD(FusedOptimizer):
+    """SGD with momentum / weight decay as one flat sm_90a kernel; gradient averaging folded in when
+    distributed.  Arithmetic = torch.optim.SGD (torch/optim/sgd.py:343-380) with dampening 0, Nesterov per group."""
+
+    def __init__(self, params, lr=1e-3, momentum=0.0, weight_decay=0.0, nesterov=False, model: nn.Module | None = None):
+        if nesterov and momentum <= 0:
+            raise ValueError("Nesterov momentum requires a momentum and zero dampening")     # torch.optim.SGD's rule
+        defaults = dict(lr=lr, momentum=momentum, weight_decay=weight_decay, nesterov=bool(nesterov), dampening=0)
+        super().__init__(params, defaults, model)
+
+    def _state_buffers(self):
+        return [self.flat.mom]
+
+    def _segment(self, b, e, g, flags):
+        if g is None:
+            return _lib.sod_sgd_segment(b, e, 0.0, 0.0, 0.0, flags)
+        if g.get("nesterov"):
+            flags |= _lib.SOD_SEG_NESTEROV
+        return _lib.sod_sgd_segment(b, e, float(g["lr"]), float(g["weight_decay"]), float(g["momentum"]), flags)
+
+    def _launch_local(self, segs, n, lr_dev, g16, s16, finf):
+        f = self.flat
+        rc = _lib.lib().sod_sgd_momentum(f.param.data_ptr(), f.mom.data_ptr(), f.grad.data_ptr(), g16, s16, f.numel,
+                                         segs, n, lr_dev, float(self.inv_scale), finf, _lib.SOD_SGD_ZERO_GRAD,
+                                         _lib.stream_ptr())
+        _lib.check(rc, "sod_sgd_momentum")
+
+    def _launch_allreduce(self, segs, n, lr_dev, g16, s16, finf):
+        f = self.flat
+        rc = _lib.lib().sod_allreduce_sgd(f.arena.ref, f.grad_off, f.grad16_off if g16 is not None else 0, f.param_off,
+                                          f.mom.data_ptr(), s16, f.numel, segs, n, lr_dev, float(self.inv_scale), finf,
+                                          _lib.SOD_SGD_ZERO_GRAD, _lib.stream_ptr())
+        _lib.check(rc, "sod_allreduce_sgd")
+
+    def gather_momentum(self) -> None:
+        """world > 1: the full momentum buffer on every rank (collective; see `gather_state`)"""
+        self.gather_state()
 
     # momentum lives in the flat buffer; expose torch.optim.SGD's state layout on demand
     def state_dict(self):
-        self.gather_momentum()
+        self.gather_state()
         self.state.clear()
         if self._stepped:
             for g in self.param_groups:
@@ -380,6 +452,111 @@ class FusedSGD(Optimizer):
         return super().__repr__().replace("FusedSGD", "FusedSGD[sm_90a flat]", 1)
 
 
+class FusedAdam(FusedOptimizer):
+    """torch.optim.Adam (amsgrad=False, maximize=False, L2 weight decay) as one flat sm_90a kernel, gradient averaging
+    folded in when distributed — the optimizer of the reference's optim "adam" (utils/pipeline_ops.py:287-294).
+    `flat.mom` holds exp_avg, `exp_avg_sq` sits beside it; the step count of every segment lives on the device
+    (`step_dev`) and is advanced by the kernel, so a captured iteration replays with the right bias correction and an
+    amp-overflow skip leaves it alone."""
+
+    def __init__(self, params, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0, amsgrad=False, *,
+                 maximize=False, decoupled_weight_decay=False, model: nn.Module | None = None, **_ignored):
+        if amsgrad or maximize or decoupled_weight_decay:
+            raise _lib.SodError("FusedAdam implements Adam without amsgrad, maximize or decoupled weight decay "
+                                "(the reference's optim 'adam' sets none of them)")
+        if not 0.0 <= betas[0] < 1.0 or not 0.0 <= betas[1] < 1.0 or eps < 0.0:
+            raise ValueError(f"invalid betas {betas} or eps {eps}")
+        defaults = dict(lr=lr, betas=tuple(betas), eps=eps, weight_decay=weight_decay, amsgrad=False, maximize=False,
+                        foreach=None, capturable=False, differentiable=False, fused=None, decoupled_weight_decay=False)
+        super().__init__(params, defaults, model)
+        self.exp_avg_sq = torch.zeros_like(self.flat.mom)
+        # int32[SOD_ADAM_STEP_WORDS]: the step count of every segment of _segment_plan(), then the kernel's ticket word
+        self.step_dev = torch.zeros(_lib.SOD_ADAM_STEP_WORDS, dtype=torch.int32, device=self.flat.device)
+
+    @property
+    def exp_avg(self) -> torch.Tensor:
+        return self.flat.mom
+
+    def _state_buffers(self):
+        return [self.flat.mom, self.exp_avg_sq]
+
+    def _snapshot_tensors(self):
+        return super()._snapshot_tensors() + [self.step_dev]
+
+    def _segment(self, b, e, g, flags):
+        if g is None:
+            return _lib.sod_adam_segment(b, e, 0.0, 0.0, 0.0, 0.0, 0.0, flags)
+        b1, b2 = g["betas"]
+        return _lib.sod_adam_segment(b, e, float(g["lr"]), float(g["weight_decay"]), float(b1), float(b2), float(g["eps"]),
+                                     flags)
+
+    def _launch_local(self, segs, n, lr_dev, g16, s16, finf):
+        f = self.flat
+        rc = _lib.lib().sod_adam(f.param.data_ptr(), f.mom.data_ptr(), self.exp_avg_sq.data_ptr(), f.grad.data_ptr(), g16,
+                                 s16, f.numel, segs, n, lr_dev, self.step_dev.data_ptr(), float(self.inv_scale), finf,
+                                 _lib.SOD_SGD_ZERO_GRAD, _lib.stream_ptr())
+        _lib.check(rc, "sod_adam")
+
+    def _launch_allreduce(self, segs, n, lr_dev, g16, s16, finf):
+        f = self.flat
+        rc = _lib.lib().sod_allreduce_adam(f.arena.ref, f.grad_off, f.grad16_off if g16 is not None else 0, f.param_off,
+                                           f.mom.data_ptr(), self.exp_avg_sq.data_ptr(), s16, f.numel, segs, n, lr_dev,
+                                           self.step_dev.data_ptr(), float(self.inv_scale), finf, _lib.SOD_SGD_ZERO_GRAD,
+                                           _lib.stream_ptr())
+        _lib.check(rc, "sod_allreduce_adam")
+
+    def group_steps(self) -> list[int]:
+        """the step count of every param_group (host sync)"""
+        steps = self.step_dev.tolist()
+        return [steps[idx[0]] if idx else 0 for idx in self._group_segments()]
+
+    # the state lives in the flat buffers; expose torch.optim.Adam's layout on demand
+    def state_dict(self):
+        self.gather_state()
+        self.state.clear()
+        for g, t in zip(self.param_groups, self.group_steps()):
+            if t == 0:
+                continue                       # torch creates a parameter's state at its first step
+            for p in g["params"]:
+                self.state[p] = {"step": torch.tensor(float(t), dtype=torch.float32),
+                                 "exp_avg": self.flat.momentum_view(p).clone(),
+                                 "exp_avg_sq": FlatParams._view(self.exp_avg_sq, self.flat.offset_of(p), p.data).clone()}
+        sd = super().state_dict()
+        self.state.clear()
+        return sd
+
+    def load_state_dict(self, state_dict):
+        """torch.optim.Adam's layout; `step` may be a tensor or (torch of 2020, which the reference ran) an int"""
+        super().load_state_dict(state_dict)
+        try:
+            steps = []
+            for g in self.param_groups:
+                ts = {int(float(self.state[p]["step"])) if "step" in self.state.get(p, {}) else 0 for p in g["params"]}
+                if len(ts) > 1:
+                    raise _lib.SodError(f"the parameters of one group carry different Adam steps {sorted(ts)}: the fused "
+                                        "step keeps one count per group")
+                steps.append(ts.pop() if ts else 0)
+            with torch.no_grad():
+                for g in self.param_groups:
+                    for p in g["params"]:
+                        st = self.state.get(p, {})
+                        if "exp_avg" in st:
+                            self.flat.momentum_view(p).copy_(st["exp_avg"])
+                            FlatParams._view(self.exp_avg_sq, self.flat.offset_of(p), p.data).copy_(st["exp_avg_sq"])
+                counts = [0] * _lib.SOD_ADAM_STEP_WORDS
+                for idx, t in zip(self._group_segments(), steps):
+                    for n in idx:
+                        counts[n] = t
+                self.step_dev.copy_(torch.tensor(counts, dtype=torch.int32))
+        finally:
+            self.state.clear()
+        self._stepped = self._stepped or any(steps)
+        self.flat.refresh_shadow()
+
+    def __repr__(self):
+        return super().__repr__().replace("FusedAdam", "FusedAdam[sm_90a flat]", 1)
+
+
 def make_optimizer(model: nn.Module, optimizer_type: str, optimizer_info: dict) -> Optimizer:
     """Parameter grouping rules of reference utils/pipeline_ops.py:235-316, FusedSGD underneath."""
     lr, mom = optimizer_info["lr"], optimizer_info["momentum"]
@@ -397,7 +574,7 @@ def make_optimizer(model: nn.Module, optimizer_type: str, optimizer_info: dict) 
     if optimizer_type == "sgd_all":
         return FusedSGD([p for _, p in named], lr=lr, weight_decay=wd, momentum=mom, model=model)
     if optimizer_type == "adam":
-        return Adam(model.parameters(), lr=lr, betas=(0.9, 0.999), eps=1e-8, weight_decay=wd)
+        return FusedAdam(model.parameters(), lr=lr, betas=(0.9, 0.999), eps=1e-8, weight_decay=wd, model=model)
     if optimizer_type == "f3_trick":
         backbone = [p for n, p in named if n.startswith("div") and not n.startswith("div_2")]
         head = [p for n, p in named if not n.startswith("div")]

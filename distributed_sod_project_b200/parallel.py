@@ -7,9 +7,9 @@ rank start from rank 0's parameters and buffers.
 Changed by design: apex flattens all gradients at the end of backward, calls NCCL all-reduce, divides by the
 world size and unflattens (four full passes over 99.6 MB plus the collective).  Here the gradients are *born*
 in one flat symmetric-memory buffer (each `.grad` is a view), and the averaging is folded into the optimizer
-step kernel (`sod_allreduce_sgd`, csrc/sgd.cu): reduce-scatter over NVSwitch → SGD on the owned shard →
-all-gather of the updated parameters.  `delay_allreduce=True` semantics hold trivially: nothing is exchanged
-before backward has finished.  With an optimizer other than FusedSGD the wrapper falls back to an explicit
+step kernel (`sod_allreduce_sgd` / `sod_allreduce_adam`, csrc/sgd.cu): reduce-scatter over NVSwitch → SGD or Adam
+on the owned shard → all-gather of the updated parameters.  `delay_allreduce=True` semantics hold trivially: nothing is
+exchanged before backward has finished.  With an optimizer other than FusedSGD / FusedAdam the wrapper falls back to an explicit
 in-place peer-memory all-reduce of the flat gradient buffer at the end of backward (`sod_allreduce_f32`).
 """
 from __future__ import annotations
@@ -19,11 +19,11 @@ import torch.nn as nn
 from torch.autograd import Variable
 
 from . import comm
-from .optim import FlatParams, FusedSGD, flat_registry as _flat_registry
+from .optim import FlatParams, FusedOptimizer, flat_registry as _flat_registry
 
 
 class DistributedDataParallel(nn.Module):
-    def __init__(self, module: nn.Module, delay_allreduce: bool = True, optimizer: FusedSGD | None = None,
+    def __init__(self, module: nn.Module, delay_allreduce: bool = True, optimizer: FusedOptimizer | None = None,
                  process_group=None, **_ignored):
         super().__init__()
         self.module = module
@@ -74,7 +74,7 @@ class DistributedDataParallel(nn.Module):
         """Materialise the averaged gradients in place (what apex leaves in `.grad` after backward)."""
         if self.world == 1:
             return
-        # an optimizer that is not FusedSGD may have dropped the bound views (torch's zero_grad(set_to_none=True) is the
+        # an optimizer that is not a fused one may have dropped the bound views (torch's zero_grad(set_to_none=True) is the
         # default): autograd then produced fresh .grad tensors OUTSIDE the symmetric buffer.  Fold them in and rebind,
         # so that what is averaged is what backward computed.
         import torch

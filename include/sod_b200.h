@@ -27,7 +27,7 @@ extern "C" {
 #define SOD_MAX_WORLD 8
 #define SOD_MAX_SEGMENTS 16
 #define SOD_COMM_MAX_BLOCKS 1024   /* flag rows per channel */
-#define SOD_COMM_CHANNELS 4        /* barrier channels: 0 gradient reduce+SGD, 3 plain all-reduce (1,2 reserved; the
+#define SOD_COMM_CHANNELS 4        /* barrier channels: 0 gradient reduce+SGD or +Adam, 3 plain all-reduce (1,2 reserved; the
                                       SyncBN exchange uses tagged packets, not flags) */
 
 typedef enum { SOD_F32 = 0, SOD_BF16 = 1, SOD_F16 = 2 } sod_dtype;
@@ -113,7 +113,9 @@ size_t sod_comm_flag_bytes(void);
  * ------------------------------------------------------------------------------------------------ */
 enum { SOD_SEG_FROZEN = 1,
        SOD_SEG_GRAD16 = 2 /* the gradient of this range exists ONLY in the bf16 buffer (`grad16`): the fp32 buffer is neither read
-                             nor cleared there, and with world>1 the bf16 values themselves cross NVLink (summed in fp32) */ };
+                             nor cleared there, and with world>1 the bf16 values themselves cross NVLink (summed in fp32) */,
+       SOD_SEG_NESTEROV = 4 /* SGD only: Nesterov momentum, v = mu*v + g ; p -= lr*(g + mu*v) (torch.optim.SGD nesterov=True,
+                               the reference's `nesterov` key for sgd_trick / f3_trick, utils/pipeline_ops.py:258,312) */ };
 typedef struct {
     int64_t begin, end;        /* element range, multiples of 4 */
     float lr, weight_decay, momentum;
@@ -143,6 +145,37 @@ int sod_sgd_momentum(float* param, float* mom, float* grad, void* grad16, void* 
 int sod_allreduce_sgd(const sod_comm* comm, uint64_t grad_off, uint64_t grad16_off, uint64_t param_off, float* mom,
                       void* shadow16, int64_t n, const sod_sgd_segment* segs, int nseg, const float* lr_dev,
                       float inv_scale, const uint32_t* found_inf, int flags, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * (1b) gradient all-reduce ⊕ unscale ⊕ Adam — the same two kernels as above with the update rule of
+ *      torch.optim.Adam (amsgrad=False, maximize=False, L2 weight decay folded into g), which the reference builds
+ *      for optim "adam" (utils/pipeline_ops.py:287-294).  Per element, with t = step_dev[segment] + 1:
+ *   g = (Σ_ranks grad) * inv_scale / world + wd*p ;  m += (1-β1)*(g-m) ;  v = β2*v + (1-β2)*g*g
+ *   p -= fp32(lr / (1-β1^t)) * m / (sqrt(v) / fp32(sqrt(1-β2^t)) + eps)      (bias corrections in fp64)
+ * exp_avg (m) and exp_avg_sq (v) are local fp32 buffers of n elements, laid out like `param`; with world>1 rank r
+ * only reads and writes its shard of them.  Everything else — segments, SOD_SEG_FROZEN / SOD_SEG_GRAD16, grad16,
+ * shadow16, lr_dev, found_inf, flags, the arena offsets — means what it means for the SGD entry points above.
+ * step_dev (device, int32[SOD_ADAM_STEP_WORDS], zeroed once by the caller): step_dev[i] is the number of steps segment i
+ * has taken; the last CTA of the launch advances every non-frozen segment's count, so a captured CUDA graph replays
+ * with the right bias correction.  When *found_inf != 0 nothing but the gradients changes (the counts included).
+ * step_dev[SOD_MAX_SEGMENTS] is a ticket word the kernel uses and leaves at 0.  One step_dev per stream at a time.
+ * SOD_SEG_NESTEROV is refused here (SOD_EINVAL), as are β outside [0, 1) and eps < 0.  β1 and β2 enter the
+ * arithmetic as the shortest decimal that rounds to the given fp32 value (0.999f → 0.999), as torch's Python floats do.
+ * ------------------------------------------------------------------------------------------------ */
+#define SOD_ADAM_STEP_WORDS (SOD_MAX_SEGMENTS + 1)
+typedef struct {
+    int64_t begin, end;        /* element range, multiples of 4 */
+    float lr, weight_decay, beta1, beta2, eps;
+    int32_t flags;
+} sod_adam_segment;
+int sod_adam(float* param, float* exp_avg, float* exp_avg_sq, float* grad, void* grad16, void* shadow16, int64_t n,
+             const sod_adam_segment* segs, int nseg, const float* lr_dev, int32_t* step_dev,
+             float inv_scale, const uint32_t* found_inf, int flags, void* stream);
+int sod_allreduce_adam(const sod_comm* comm, uint64_t grad_off, uint64_t grad16_off, uint64_t param_off,
+                       float* exp_avg, float* exp_avg_sq, void* shadow16, int64_t n, const sod_adam_segment* segs,
+                       int nseg, const float* lr_dev, int32_t* step_dev, float inv_scale,
+                       const uint32_t* found_inf, int flags, void* stream);
+
 /* Multi-tensor gather of bf16 gradients into the flat bf16 gradient buffer (`grad16` above): item i copies
  * numel elements from the dense tensor `src` to dst16[dst_offset ...] (dst_offset % 8 == 0).  Replaces the
  * per-parameter accumulate kernels autograd launches at the end of backward (train.py:302): the weight gradients are
