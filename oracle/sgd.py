@@ -3,7 +3,7 @@ gradient unscale, and the flat all-reduce-mean that precedes it.
 
 Follows
 * `torch.optim.SGD` single-tensor math — torch/optim/sgd.py:343-380 (weight decay folded into the
-  gradient, `buf = g` on the first step else `buf = mu*buf + g`, dampening 0, no nesterov), as
+  gradient, `buf = g` on the first step else `buf = mu*buf + g`, dampening 0; Nesterov in `sgd_step_f64` only), as
   configured by the reference `make_optimizer(..., "f3_trick")` — utils/pipeline_ops.py:295-313
   (backbone lr×0.1, head lr×1, names starting with `div_2` in no group), stepped at train.py:303;
 * apex `DistributedDataParallel(delay_allreduce=True)` published semantics (train.py:185): one flat
@@ -29,6 +29,7 @@ class Segment:
     weight_decay: float
     momentum: float = 0.9
     frozen: bool = False    # True: gradients are still averaged, but p / v are not touched (div_2.*)
+    nesterov: bool = False  # torch.optim.SGD(nesterov=True): p -= lr*(g + mu*v) after the momentum update
 
 
 def allreduce_mean(rank_grads: list[np.ndarray]) -> np.ndarray:
@@ -42,8 +43,10 @@ def allreduce_mean(rank_grads: list[np.ndarray]) -> np.ndarray:
 
 def sgd_step(p: np.ndarray, v: np.ndarray, g: np.ndarray, segments: list[Segment],
              inv_scale: float = 1.0) -> bool:
-    """In-place fp32 step. Returns False (and touches nothing) when a gradient is non-finite
-    (the amp overflow-skip)."""
+    """In-place fp32 step of plain momentum (a Nesterov segment raises: `sgd_step_f64` restates it).  Returns False
+    (and touches nothing) when a gradient is non-finite (the amp overflow-skip)."""
+    if any(s.nesterov for s in segments):
+        raise NotImplementedError("sgd_step restates plain momentum only; use sgd_step_f64 for Nesterov segments")
     if not np.all(np.isfinite(g)):
         return False
     f = np.float32
@@ -66,7 +69,7 @@ def sgd_step_f64(p, v, g, segments, inv_scale=1.0):
         sl = slice(s.begin, s.end)
         gg = g[sl] * inv_scale + s.weight_decay * p[sl]
         v[sl] = s.momentum * v[sl] + gg
-        p[sl] = p[sl] - s.lr * v[sl]
+        p[sl] = p[sl] - s.lr * (gg + s.momentum * v[sl] if s.nesterov else v[sl])
     return p, v
 
 
