@@ -25,7 +25,9 @@ SOD_BN_BWD_MASK_FROM_X = 32
 SOD_BN_L2_HINTS = 64
 SOD_BN_LAUNCH_COOP = 128
 SOD_BN_LAUNCH_PDL = 256
+SOD_GRAD16_F16 = 512
 SOD_GATHER_MAX_ITEMS = 160
+SOD_CHECK_MAX_RANGES = 128
 SOD_ADAM_STEP_WORDS = SOD_MAX_SEGMENTS + 1
 ABI_VERSION = 7
 
@@ -54,6 +56,18 @@ class sod_adam_segment(C.Structure):
                 ("beta1", C.c_float), ("beta2", C.c_float), ("eps", C.c_float), ("flags", C.c_int32)]
 
 
+class sod_loss_scaler(C.Structure):
+    _fields_ = [("found_inf", C.c_uint32), ("scale", C.c_float), ("unskipped", C.c_int32), ("growth_interval", C.c_int32),
+                ("ticket", C.c_uint32), ("reserved", C.c_uint32 * 3)]
+
+
+SOD_LOSS_SCALER_WORDS = 8     # sizeof(sod_loss_scaler) / 4: [found_inf, scale (fp32 bits), unskipped, growth_interval, ticket, …]
+
+
+class sod_check_range(C.Structure):
+    _fields_ = [("begin", C.c_int64), ("end", C.c_int64), ("flags", C.c_int32)]
+
+
 _PROTOTYPES = {
     "sod_version": (C.c_int, []),
     "sod_strerror": (C.c_char_p, [C.c_int]),
@@ -62,6 +76,9 @@ _PROTOTYPES = {
     "sod_loss_bce_cel_fwd_bwd": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p,
                                            C.c_int64, C.c_int, C.c_float, C.c_float, C.c_float, C.c_float, C.c_int,
                                            C.c_void_p, C.c_size_t, C.c_void_p]),
+    "sod_loss_bce_cel_fwd_bwd_scaled": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p,
+                                                  C.c_int64, C.c_int, C.c_float, C.c_float, C.c_float, C.c_void_p, C.c_float,
+                                                  C.c_int, C.c_void_p, C.c_size_t, C.c_void_p]),
     "sod_scale_by_device_scalar": (C.c_int, [C.c_void_p, C.c_int, C.c_int64, C.c_void_p, C.c_void_p]),
     "sod_comm_flag_bytes": (C.c_size_t, []),
     "sod_sgd_momentum": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
@@ -74,9 +91,24 @@ _PROTOTYPES = {
     "sod_allreduce_adam": (C.c_int, [C.POINTER(sod_comm), C.c_uint64, C.c_uint64, C.c_uint64, C.c_void_p, C.c_void_p,
                                      C.c_void_p, C.c_int64, C.POINTER(sod_adam_segment), C.c_int, C.c_void_p, C.c_void_p,
                                      C.c_float, C.c_void_p, C.c_int, C.c_void_p]),
+    "sod_sgd_momentum_scaler": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
+                                          C.POINTER(sod_sgd_segment), C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
+    "sod_allreduce_sgd_scaler": (C.c_int, [C.POINTER(sod_comm), C.c_uint64, C.c_uint64, C.c_uint64, C.c_void_p, C.c_void_p,
+                                           C.c_int64, C.POINTER(sod_sgd_segment), C.c_int, C.c_void_p, C.c_void_p, C.c_int,
+                                           C.c_void_p]),
+    "sod_adam_scaler": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
+                                  C.POINTER(sod_adam_segment), C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
+    "sod_allreduce_adam_scaler": (C.c_int, [C.POINTER(sod_comm), C.c_uint64, C.c_uint64, C.c_uint64, C.c_void_p, C.c_void_p,
+                                            C.c_void_p, C.c_int64, C.POINTER(sod_adam_segment), C.c_int, C.c_void_p, C.c_void_p,
+                                            C.c_void_p, C.c_int, C.c_void_p]),
     "sod_grad_gather16": (C.c_int, [C.POINTER(sod_gather_item), C.c_int, C.c_void_p, C.c_int64, C.c_void_p]),
+    "sod_grad_gather16_checked": (C.c_int, [C.POINTER(sod_gather_item), C.c_int, C.c_void_p, C.c_int64, C.c_int, C.c_void_p,
+                                            C.c_void_p]),
     "sod_grad_merge_bf16": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
+    "sod_grad_merge16": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p]),
     "sod_grad_nonfinite": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
+    "sod_grad_check_ranges": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.POINTER(sod_check_range), C.c_int, C.c_int,
+                                        C.c_void_p, C.c_void_p]),
     "sod_allreduce_f32": (C.c_int, [C.POINTER(sod_comm), C.c_uint64, C.c_int64, C.c_float, C.c_int, C.c_int, C.c_void_p]),
     "sod_syncbn_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int]),
     "sod_syncbn_exchange_bytes": (C.c_size_t, [C.c_int]),

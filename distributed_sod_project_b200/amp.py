@@ -4,8 +4,14 @@
 Default: bf16 autocast, loss scale fixed at 1.0 — bf16 has fp32's exponent range, so the dynamic
 scaler of apex O1 has nothing to do; weights, gradients and optimizer state stay fp32 ("fp32 master") exactly
 as under O1.  `dtype=torch.float16` keeps apex's dynamic-scale behaviour (init 2^16, ÷2 and skip the step on
-overflow, ×2 every 2000 clean steps): the unscale factor and the overflow flag are consumed INSIDE the fused
-optimizer kernel, the only extra work is one read of the gradients by `sod_grad_nonfinite`.
+overflow, never below 1, ×2 after every `growth_interval` (2000) clean steps in a row).  The scaler lives on the device
+(`sod_loss_scaler`, include/sod_b200.h): the loss gradient is formed already scaled, the overflow checks ride on the
+gradient gather, and the fused step kernel reads the verdict and 1/scale and advances the scaler itself — so an fp16
+iteration has no host round trip and replays from a CUDA graph like a bf16 one.  Both dtypes use the 16-bit shadow weights.
+
+`_cfg["scale"]` / `_cfg["good_steps"]` are a host mirror of the device scaler: an eager step reads it back (the one host
+sync that path makes anyway), a graph replay does not (`read_scaler()` does, on demand); a host write to `_cfg["scale"]`,
+`_cfg["good_steps"]` or `_cfg["growth_interval"]` is pushed to the device before the next iteration.
 """
 from __future__ import annotations
 
@@ -23,13 +29,15 @@ import os
 STEAL_WEIGHT_GRADS = os.environ.get("SOD_STEAL_WGRADS", "1") == "1"
 
 _cfg = {"enabled": False, "dtype": torch.bfloat16, "scale": 1.0, "dynamic": False, "good_steps": 0,
-        "growth_interval": 2000, "found_inf": None}
+        "growth_interval": 2000, "owner": None, "dev": None}
+# owner: the FusedOptimizer whose flat buffers hold the device scaler (fp16 only); dev: the mirror values last known to be
+# on the device, {"scale", "good_steps", "growth_interval"} — a host value that differs from it is pushed
 
 
 def _install_shadow_weights(model, flat) -> int:
-    """Point every Conv2d whose parameters live in `flat` at the bf16 shadow copy: under autocast the convolution
-    then takes its weight without a per-iteration cast kernel, and autograd accumulates the (bf16) weight gradient
-    straight into the flat bf16 gradient buffer the fused step consumes.  fp32 masters stay the module Parameters
+    """Point every Conv2d whose parameters live in `flat` at the 16-bit (bf16 or fp16) shadow copy: under autocast the
+    convolution then takes its weight without a per-iteration cast kernel, and autograd accumulates the 16-bit weight
+    gradient straight into the flat 16-bit gradient buffer the fused step consumes.  fp32 masters stay the module Parameters
     (state_dict / checkpoints / optimizer groups are unaffected)."""
     import torch.nn as nn
     managed = {id(p) for p, _ in flat.slots}
@@ -91,6 +99,8 @@ def initialize(model, optimizer=None, opt_level: str = "O1", dtype: torch.dtype 
     _cfg["dtype"] = dtype
     _cfg["dynamic"] = _cfg["enabled"] and dtype == torch.float16
     _cfg["scale"] = 65536.0 if _cfg["dynamic"] else 1.0
+    _cfg["good_steps"] = 0
+    _cfg["owner"] = _cfg["dev"] = None
     if _cfg["enabled"]:
         inner = model.forward
 
@@ -100,44 +110,87 @@ def initialize(model, optimizer=None, opt_level: str = "O1", dtype: torch.dtype 
                 return inner(*a, **k)
 
         model.forward = autocast_forward
-        if shadow_weights and dtype == torch.bfloat16 and isinstance(optimizer, FusedOptimizer) and optimizer.flat.param.is_cuda:
+        fused_cuda = isinstance(optimizer, FusedOptimizer) and optimizer.flat.param.is_cuda
+        if _cfg["dynamic"] and fused_cuda:
+            optimizer.flat.enable_scaler(_cfg["scale"], _cfg["growth_interval"])
+            _cfg["owner"] = optimizer
+            _cfg["dev"] = {k: _cfg[k] for k in ("scale", "good_steps", "growth_interval")}
+            optimizer._scaler_readback = _read_back
+        if shadow_weights and dtype in (torch.bfloat16, torch.float16) and fused_cuda:
             optimizer.flat.enable_shadow(dtype)
             _install_shadow_weights(model, optimizer.flat)
     return (model, optimizer) if optimizer is not None else model
 
 
+def _scaler() -> torch.Tensor | None:
+    """the device scaler (int32[SOD_LOSS_SCALER_WORDS], `sod_loss_scaler`), or None when the loss scale is static"""
+    owner = _cfg.get("owner")
+    return owner.flat.scaler if (_cfg["dynamic"] and owner is not None) else None
+
+
+def scale_tensor() -> torch.Tensor | None:
+    """0-d fp32 view of the device loss scale (what `scale_loss` multiplies the loss by and the fused loss kernel scales its
+    gradient by), or None when the loss scale is static"""
+    s = _scaler()
+    return s.view(torch.float32)[1] if s is not None else None
+
+
+def push() -> None:
+    """bring host writes of `_cfg["scale"]` / `["good_steps"]` / `["growth_interval"]` to the device scaler (stream-ordered
+    fills, no sync; a no-op when nothing changed and while a CUDA graph is being captured)"""
+    s = _scaler()
+    if s is None or torch.cuda.is_current_stream_capturing():
+        return
+    dev = _cfg["dev"]
+    if _cfg["scale"] != dev["scale"]:
+        s.view(torch.float32)[1].fill_(float(_cfg["scale"]))
+    if _cfg["good_steps"] != dev["good_steps"]:
+        s[2].fill_(int(_cfg["good_steps"]))
+    if _cfg["growth_interval"] != dev["growth_interval"]:
+        s[3].fill_(int(_cfg["growth_interval"]))
+    _cfg["dev"] = {k: _cfg[k] for k in ("scale", "good_steps", "growth_interval")}
+
+
+def _read_back() -> None:
+    s = _scaler()
+    if s is None:
+        return
+    w = s[:4].cpu()                                        # one 16-byte D2H copy (host sync)
+    _cfg["scale"] = float(w.view(torch.float32)[1])
+    _cfg["good_steps"] = int(w[2])
+    _cfg["growth_interval"] = int(w[3])
+    _cfg["dev"] = {k: _cfg[k] for k in ("scale", "good_steps", "growth_interval")}
+
+
+def read_scaler() -> dict:
+    """the device scaler as the host sees it after a sync — {"scale", "unskipped", "found_inf"} — and the host mirror
+    brought up to date (after graph replays, which do not update it)"""
+    s = _scaler()
+    if s is None:
+        return {"scale": _cfg["scale"], "unskipped": _cfg["good_steps"], "found_inf": 0}
+    push()
+    _read_back()
+    return {"scale": _cfg["scale"], "unskipped": _cfg["good_steps"], "found_inf": int(s[0].item())}
+
+
 @contextlib.contextmanager
 def scale_loss(loss, optimizer):
-    """`with amp.scale_loss(loss, optimizer) as scaled: scaled.backward()` (reference train.py:299)."""
+    """`with amp.scale_loss(loss, optimizer) as scaled: scaled.backward()` (reference train.py:299).  fp16: yields
+    loss × the device scale; the overflow check, the skip and the scale update happen inside `optimizer.step()`."""
     if not _cfg["dynamic"]:
         yield loss
         return
     if not isinstance(optimizer, FusedOptimizer):
         raise _lib.SodError("fp16 dynamic loss scaling is wired into the fused optimizers (FusedSGD, FusedAdam) only")
-    scale = _cfg["scale"]
-    yield loss * scale
-    flat = optimizer.flat
-    if _cfg["found_inf"] is None:
-        _cfg["found_inf"] = torch.zeros(1, dtype=torch.int32, device=flat.grad.device)
-    finf = _cfg["found_inf"]
-    finf.zero_()
-    rc = _lib.lib().sod_grad_nonfinite(flat.grad.data_ptr(), flat.numel, finf.data_ptr(), _lib.stream_ptr())
-    _lib.check(rc, "sod_grad_nonfinite")
-    _lib.count_launch()
-    if flat.arena is not None:
-        torch.distributed.all_reduce(finf, op=torch.distributed.ReduceOp.MAX)   # identical verdict on all ranks
-    optimizer.inv_scale = 1.0 / scale
-    optimizer.found_inf = finf
-    if int(finf.item()):                       # apex syncs here too
-        _cfg["scale"] = max(scale / 2.0, 1.0)
-        _cfg["good_steps"] = 0
-    else:
-        _cfg["good_steps"] += 1
-        if _cfg["good_steps"] % _cfg["growth_interval"] == 0:
-            _cfg["scale"] = scale * 2.0
+    if optimizer is not _cfg["owner"] or optimizer.flat.scaler is None:
+        raise _lib.SodError("fp16 dynamic loss scaling needs the optimizer that was passed to amp.initialize (on CUDA)")
+    push()
+    yield loss * scale_tensor()
 
 
 def state_dict():
+    if _scaler() is not None:
+        read_scaler()
     return {"loss_scaler0": {"loss_scale": _cfg["scale"], "unskipped": _cfg["good_steps"]}}
 
 
@@ -145,3 +198,4 @@ def load_state_dict(sd):
     s = sd.get("loss_scaler0", {})
     _cfg["scale"] = float(s.get("loss_scale", _cfg["scale"]))
     _cfg["good_steps"] = int(s.get("unskipped", 0))
+    push()

@@ -36,7 +36,14 @@ struct LossParams {
     int resident;       // chunks held in shared memory per CTA
     int reduction_sum;
     float w_bce, w_cel, grad_scale, eps;
+    const float* grad_scale_dev;  // amp loss scale (device scalar) multiplying grad_scale, or NULL
 };
+
+// grad_scale, times the device-resident amp loss scale when there is one: it enters kb, α and β, so every gradient is
+// rounded to the logits dtype once, already scaled
+__device__ __forceinline__ float effective_grad_scale(const LossParams& prm) {
+    return prm.grad_scale_dev != nullptr ? prm.grad_scale * *prm.grad_scale_dev : prm.grad_scale;
+}
 
 // d = p(1-t) + t(1-p) = |p - t| for a binary t: CEL's numerator term.  It is summed as such, never formed as
 // Σp + Σt - 2Σpt, which cancels when the predictions are confident and p ≈ t (late in training).
@@ -184,9 +191,10 @@ __global__ void __launch_bounds__(kThreads, 1) loss_bce_cel_kernel(const LossPar
         o[7] = static_cast<float>(n);
     }
     // d total/dx = kb (p-t) + w_cel gs p(1-p) [ (1-2t)/den - num/den^2 ]
-    const float kb = prm.grad_scale * prm.w_bce * (prm.reduction_sum ? 1.0f : static_cast<float>(1.0 / static_cast<double>(n)));
-    const float alpha = static_cast<float>(static_cast<double>(prm.grad_scale) * prm.w_cel / den);
-    const float beta = static_cast<float>(-static_cast<double>(prm.grad_scale) * prm.w_cel * num / (den * den));
+    const float gs = effective_grad_scale(prm);
+    const float kb = gs * prm.w_bce * (prm.reduction_sum ? 1.0f : static_cast<float>(1.0 / static_cast<double>(n)));
+    const float alpha = static_cast<float>(static_cast<double>(gs) * prm.w_cel / den);
+    const float beta = static_cast<float>(-static_cast<double>(gs) * prm.w_cel * num / (den * den));
 
     // ---- phase 2: gradients, re-reading the slice from shared memory --------------------------------
     for (int c = 0; c < nchunks; ++c) {
@@ -342,9 +350,10 @@ __global__ void __launch_bounds__(kStreamBlock, 1) loss_stream_kernel(const Loss
         o[3] = static_cast<float>(sp); o[4] = static_cast<float>(st); o[5] = static_cast<float>(spt);
         o[6] = static_cast<float>(bce_sum); o[7] = static_cast<float>(n);
     }
-    const float kb = prm.grad_scale * prm.w_bce * (prm.reduction_sum ? 1.0f : static_cast<float>(1.0 / static_cast<double>(n)));
-    const float alpha = static_cast<float>(static_cast<double>(prm.grad_scale) * prm.w_cel / den);
-    const float beta = static_cast<float>(-static_cast<double>(prm.grad_scale) * prm.w_cel * num / (den * den));
+    const float gs = effective_grad_scale(prm);
+    const float kb = gs * prm.w_bce * (prm.reduction_sum ? 1.0f : static_cast<float>(1.0 / static_cast<double>(n)));
+    const float alpha = static_cast<float>(static_cast<double>(gs) * prm.w_cel / den);
+    const float beta = static_cast<float>(-static_cast<double>(gs) * prm.w_cel * num / (den * den));
 
     // ---- phase 2: resident chunks first, then the re-streamed ones (newest first) ----------------------------------
     const int nresident = nchunks - nres0;
@@ -446,6 +455,16 @@ extern "C" int sod_loss_bce_cel_fwd_bwd(const void* logits, int logits_dtype, co
                                         void* grad_logits, int grad_dtype, float* scalars_out, int64_t n,
                                         int reduction_sum, float w_bce, float w_cel, float grad_scale, float eps,
                                         int mode, void* workspace, size_t workspace_bytes, void* stream) {
+    return sod_loss_bce_cel_fwd_bwd_scaled(logits, logits_dtype, mask, mask_dtype, grad_logits, grad_dtype, scalars_out, n,
+                                           reduction_sum, w_bce, w_cel, grad_scale, nullptr, eps, mode, workspace,
+                                           workspace_bytes, stream);
+}
+
+extern "C" int sod_loss_bce_cel_fwd_bwd_scaled(const void* logits, int logits_dtype, const void* mask, int mask_dtype,
+                                               void* grad_logits, int grad_dtype, float* scalars_out, int64_t n,
+                                               int reduction_sum, float w_bce, float w_cel, float grad_scale,
+                                               const float* grad_scale_dev, float eps, int mode, void* workspace,
+                                               size_t workspace_bytes, void* stream) {
     using namespace sod;
     SOD_CHECK_ARG(logits && mask && grad_logits && scalars_out && workspace, SOD_EINVAL);
     SOD_CHECK_ARG(n > 0 && mode >= 0 && mode <= 2, SOD_EINVAL);
@@ -460,6 +479,7 @@ extern "C" int sod_loss_bce_cel_fwd_bwd(const void* logits, int logits_dtype, co
     prm.partials = static_cast<float4*>(workspace);
     prm.n = n; prm.reduction_sum = reduction_sum ? 1 : 0;
     prm.w_bce = w_bce; prm.w_cel = w_cel; prm.grad_scale = grad_scale; prm.eps = eps;
+    prm.grad_scale_dev = grad_scale_dev;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     switch (logits_dtype) {
         case SOD_F32: return launch_loss<float, float>(prm, mode, s);

@@ -18,12 +18,15 @@
 //   all-reduce, but no separate NCCL call, no ÷W pass, no optimizer kernel, and momentum is only ever
 //   touched on the owning rank (1/W of the optimizer-state traffic; the same holds for Adam's m and v).
 // Both kernels are templates on the update rule (SgdRule / AdamRule below): the segment walk, the bf16-gradient
-// handling, the exchange and the zero-grad / shadow tail exist once.
+// handling, the exchange and the zero-grad / shadow tail exist once.  Two more template parameters: the 16-bit format of
+// grad16 / shadow16 (Bf16x4, or F16x4 for amp fp16) and whether skip and 1/scale come from the device-resident loss
+// scaler, which the kernel then advances (apex amp O1's dynamic loss scale, no host round trip).
 //   Owner-computes + broadcast also makes parameters bit-identical on all ranks by construction.
 #include "common.cuh"
 
 #include <cstdio>
 #include <cstdlib>
+#include <type_traits>
 
 namespace sod {
 namespace {
@@ -229,14 +232,76 @@ __device__ __forceinline__ uint2 f32x4_to_bf16(const float4& f) {
     return u;
 }
 
-template <class Rule>
+// The 16-bit format of `grad16` / `shadow16`, four elements per uint2, and the exponent field that marks inf / NaN:
+// bf16 (amp bf16, the default) or fp16 (SOD_GRAD16_F16, amp fp16).  Both convert with round-to-nearest-even.
+struct Bf16x4 {
+    static constexpr uint32_t kExp = 0x7f80u;
+    __device__ __forceinline__ static float4 to_f32(uint2 u) { return bf16x4_to_f32(u); }
+    __device__ __forceinline__ static uint2 from_f32(const float4& f) { return f32x4_to_bf16(f); }
+};
+struct F16x4 {
+    static constexpr uint32_t kExp = 0x7c00u;
+    __device__ __forceinline__ static float4 to_f32(uint2 u) {
+        const __half2* h = reinterpret_cast<const __half2*>(&u);
+        const float2 a = __half22float2(h[0]), b = __half22float2(h[1]);
+        return make_float4(a.x, a.y, b.x, b.y);
+    }
+    __device__ __forceinline__ static uint2 from_f32(const float4& f) {
+        uint2 u;
+        __half2* h = reinterpret_cast<__half2*>(&u);
+        h[0] = __floats2half2_rn(f.x, f.y);
+        h[1] = __floats2half2_rn(f.z, f.w);
+        return u;
+    }
+};
+
+// both 16-bit halves of w: is either inf or NaN (exponent field all ones) in the format whose exponent mask is kExp
+template <uint32_t kExp>
+__device__ __forceinline__ bool nonfinite16x2(uint32_t w) {
+    return (w & kExp) == kExp || ((w >> 16) & kExp) == kExp;
+}
+
+// The dynamic loss scale's rules (apex amp O1, include/sod_b200.h sod_loss_scaler), applied once per step by the last CTA
+// to get here (a ticket, as AdamRule::epilogue does), which then re-arms the ticket.  found_inf is left at the verdict.
+__device__ __forceinline__ void scaler_epilogue(sod_loss_scaler* sc, bool skip) {
+    __shared__ bool s_last;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        __threadfence();
+        s_last = atomicAdd(&sc->ticket, 1u) == gridDim.x - 1;
+    }
+    __syncthreads();
+    if (s_last && threadIdx.x == 0) {
+        __threadfence();
+        if (skip) {
+            sc->scale = fmaxf(sc->scale * 0.5f, 1.0f);
+            sc->unskipped = 0;
+        } else {
+            sc->unskipped += 1;
+            if (sc->growth_interval > 0 && sc->unskipped % sc->growth_interval == 0) sc->scale *= 2.0f;
+        }
+        sc->found_inf = skip ? 1u : 0u;
+        sc->ticket = 0u;
+    }
+}
+
+// kScaler: skip and 1/scale come from the device-resident loss scaler (read at execution time), which the kernel then
+// advances; otherwise from the (inv_scale, found_inf) arguments
+template <class Rule, class H, bool kScaler>
 __global__ void __launch_bounds__(kThreads) local_step_kernel(float4* __restrict__ p, const Rule rule,
                                                               float4* __restrict__ g, uint2* __restrict__ g16,
                                                               uint2* __restrict__ shadow, long long nvec,
-                                                              const __grid_constant__ SegTable segs, float inv_scale,
+                                                              const __grid_constant__ SegTable segs, float inv_scale_arg,
                                                               const uint32_t* found_inf, int zero_grad,
-                                                              const float* __restrict__ lr_dev) {
-    const bool skip = (found_inf != nullptr && *found_inf != 0);  // amp overflow: no update, but still clear g
+                                                              const float* __restrict__ lr_dev, sod_loss_scaler* scaler) {
+    bool skip;                                                     // amp overflow: no update, but still clear g
+    float inv_scale = inv_scale_arg;
+    if constexpr (kScaler) {
+        skip = scaler->found_inf != 0u;
+        inv_scale = 1.0f / scaler->scale;
+    } else {
+        skip = (found_inf != nullptr && *found_inf != 0);
+    }
     __shared__ typename Rule::Cta cta;
     rule.prologue(cta, segs, lr_dev);
     if constexpr (Rule::kHasCta) __syncthreads();
@@ -258,11 +323,11 @@ __global__ void __launch_bounds__(kThreads) local_step_kernel(float4* __restrict
                 // SOD_SEG_GRAD16: the gradient of this range exists in bf16 only — the fp32 buffer is neither read nor cleared
                 only16[u] = in_seg && g16 != nullptr && (segs.flags[cur.s] & SOD_SEG_GRAD16);
                 if (only16[u]) {
-                    gv[u] = bf16x4_to_f32(g16[i]);
+                    gv[u] = H::to_f32(g16[i]);
                 } else {
                     gv[u] = g[i];
                     if (g16 != nullptr) {   // gradients autograd left in bf16: fold them in here (the "cast" of amp O1)
-                        const float4 h = bf16x4_to_f32(g16[i]);
+                        const float4 h = H::to_f32(g16[i]);
                         gv[u].x += h.x; gv[u].y += h.y; gv[u].z += h.z; gv[u].w += h.w;
                     }
                 }
@@ -283,7 +348,7 @@ __global__ void __launch_bounds__(kThreads) local_step_kernel(float4* __restrict
                     rule.update(pv[u], st[u], gs, segs, lr_dev, cta, s);
                     p[i] = pv[u];
                     rule.store(st[u], i);
-                    if (shadow != nullptr) shadow[i] = f32x4_to_bf16(pv[u]);
+                    if (shadow != nullptr) shadow[i] = H::from_f32(pv[u]);
                 }
                 if (zero_grad) {
                     if (!only16[u]) g[i] = zero;
@@ -293,15 +358,17 @@ __global__ void __launch_bounds__(kThreads) local_step_kernel(float4* __restrict
         }
     }
     rule.epilogue(segs, skip);
+    if constexpr (kScaler) scaler_epilogue(scaler, skip);
 }
 
-__global__ void grad_merge_bf16_kernel(float4* __restrict__ g, uint2* __restrict__ g16, long long nvec) {
+template <class H>
+__global__ void grad_merge16_kernel(float4* __restrict__ g, uint2* __restrict__ g16, long long nvec) {
     for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < nvec;
          i += static_cast<long long>(gridDim.x) * blockDim.x) {
         const uint2 raw = g16[i];
         if ((raw.x | raw.y) != 0u) {   // most of the flat buffer (BN parameters, padding) never sees a bf16 gradient
             float4 a = g[i];
-            const float4 h = bf16x4_to_f32(raw);
+            const float4 h = H::to_f32(raw);
             a.x += h.x; a.y += h.y; a.z += h.z; a.w += h.w;
             g[i] = a;
             g16[i] = make_uint2(0u, 0u);
@@ -323,7 +390,11 @@ struct GatherTable {
     unsigned chunk0[kGatherMax + 1];        // prefix sum of ceil(numel / kGatherChunk)
 };
 
-__global__ void __launch_bounds__(256) grad_gather16_kernel(const __grid_constant__ GatherTable t, uint4* __restrict__ dst) {
+// kExp != 0 (sod_grad_gather16_checked): also OR into *found whether anything copied is inf / NaN in the format of kExp
+template <uint32_t kExp>
+__global__ void __launch_bounds__(256) grad_gather16_kernel(const __grid_constant__ GatherTable t, uint4* __restrict__ dst,
+                                                            uint32_t* found) {
+    bool bad = false;
     const unsigned total = t.chunk0[t.n];
     for (unsigned c = blockIdx.x; c < total; c += gridDim.x) {
         int lo = 0, hi = t.n - 1;           // item with chunk0[item] <= c < chunk0[item+1]
@@ -340,12 +411,67 @@ __global__ void __launch_bounds__(256) grad_gather16_kernel(const __grid_constan
             const uint4* s4 = reinterpret_cast<const uint4*>(src);
             uint4* d4 = reinterpret_cast<uint4*>(out);                 // dst offsets and chunk starts are multiples of 8
             const unsigned nv = cnt >> 3;
-            for (unsigned i = threadIdx.x; i < nv; i += 256) d4[i] = __ldcs(s4 + i);
-            for (unsigned i = (nv << 3) + threadIdx.x; i < cnt; i += 256) out[i] = src[i];
+            for (unsigned i = threadIdx.x; i < nv; i += 256) {
+                const uint4 v = __ldcs(s4 + i);
+                d4[i] = v;
+                if constexpr (kExp != 0u)
+                    bad |= nonfinite16x2<kExp>(v.x) | nonfinite16x2<kExp>(v.y) | nonfinite16x2<kExp>(v.z) |
+                           nonfinite16x2<kExp>(v.w);
+            }
+            for (unsigned i = (nv << 3) + threadIdx.x; i < cnt; i += 256) {
+                const unsigned short v = src[i];
+                out[i] = v;
+                if constexpr (kExp != 0u) bad |= (v & kExp) == kExp;
+            }
         } else {
-            for (unsigned i = threadIdx.x; i < cnt; i += 256) out[i] = src[i];
+            for (unsigned i = threadIdx.x; i < cnt; i += 256) {
+                const unsigned short v = src[i];
+                out[i] = v;
+                if constexpr (kExp != 0u) bad |= (v & kExp) == kExp;
+            }
         }
     }
+    if constexpr (kExp != 0u)
+        if (__syncthreads_or(bad) && threadIdx.x == 0) atomicOr(found, 1u);
+}
+
+// ------------------------------------------------------------------------------------------------
+// amp overflow check of the gradients the checked gather does not copy: listed ranges of the fp32 buffer (BN γ/β and
+// other parameters without a 16-bit gradient) and of the 16-bit one (folded convolution-bias gradients the SyncBN backward
+// accumulates in place).  Same chunked work split as the gather.
+// ------------------------------------------------------------------------------------------------
+constexpr int kCheckMax = SOD_CHECK_MAX_RANGES;
+constexpr int kCheckChunk = 4096;
+struct CheckTable {
+    int n;
+    long long begin[kCheckMax];
+    unsigned numel[kCheckMax];
+    unsigned chunk0[kCheckMax + 1];
+    unsigned char in16[kCheckMax];
+};
+
+template <uint32_t kExp>
+__global__ void __launch_bounds__(256) grad_check_ranges_kernel(const __grid_constant__ CheckTable t, const float* __restrict__ g,
+                                                                const unsigned short* __restrict__ g16, uint32_t* found) {
+    bool bad = false;
+    const unsigned total = t.chunk0[t.n];
+    for (unsigned c = blockIdx.x; c < total; c += gridDim.x) {
+        int lo = 0, hi = t.n - 1;
+        while (lo < hi) {
+            const int mid = (lo + hi + 1) >> 1;
+            if (t.chunk0[mid] <= c) lo = mid; else hi = mid - 1;
+        }
+        const unsigned first = (c - t.chunk0[lo]) * kCheckChunk;
+        const unsigned left = t.numel[lo] - first;
+        const unsigned cnt = left < kCheckChunk ? left : kCheckChunk;
+        const long long b = t.begin[lo] + first;
+        if (t.in16[lo]) {
+            for (unsigned i = threadIdx.x; i < cnt; i += 256) bad |= (g16[b + i] & kExp) == kExp;
+        } else {
+            for (unsigned i = threadIdx.x; i < cnt; i += 256) bad |= !isfinite(g[b + i]);
+        }
+    }
+    if (__syncthreads_or(bad) && threadIdx.x == 0) atomicOr(found, 1u);
 }
 
 __global__ void grad_nonfinite_kernel(const float4* __restrict__ g, long long nvec, uint32_t* found) {
@@ -384,7 +510,9 @@ __device__ __forceinline__ void broadcast_vec(const CommDev& c, uint64_t byte_of
 }
 
 // bf16 gradients on the wire: 4 elements = 8 bytes per rank, summed in fp32 in rank order (exact: no rounding of the sum,
-// unlike a bf16 multimem reduction), so every owner obtains the same value it would from an fp32 exchange of the same data
+// unlike a bf16 multimem reduction), so every owner obtains the same value it would from an fp32 exchange of the same data.
+// H = F16x4: the same for fp16 gradients (exact as well: every fp16 value is an fp32 value)
+template <class H>
 __device__ __forceinline__ float4 reduce_vec16(const CommDev& c, uint64_t byte_off) {
     float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
     uint2 raw[SOD_MAX_WORLD];
@@ -394,25 +522,43 @@ __device__ __forceinline__ float4 reduce_vec16(const CommDev& c, uint64_t byte_o
 #pragma unroll
     for (int q = 0; q < SOD_MAX_WORLD; ++q)
         if (q < c.world) {
-            const float4 t = bf16x4_to_f32(raw[q]);
+            const float4 t = H::to_f32(raw[q]);
             acc.x += t.x; acc.y += t.y; acc.z += t.z; acc.w += t.w;
         }
     return acc;
 }
 
-template <class Rule, bool kMulticast>
+// kScaler: the loss scaler sits at arena offset scaler_off on every rank; the verdict is the OR of all ranks' found_inf
+// words, read after the start barrier (each rank cleared its own before its checks, after its previous step), and the
+// scale is the local scaler's (bit-identical on all ranks, since every rank applies the same verdict)
+template <class Rule, bool kMulticast, class H, bool kScaler>
 __global__ void __launch_bounds__(kThreads) allreduce_step_kernel(const __grid_constant__ CommDev c, uint64_t grad_off,
                                                                   uint64_t param_off, const Rule rule,
                                                                   long long nvec, const __grid_constant__ SegTable segs,
-                                                                  float scale, const uint32_t* found_inf,
+                                                                  float scale_arg, const uint32_t* found_inf,
                                                                   int zero_grad, uint2* __restrict__ shadow,
                                                                   const float* __restrict__ lr_dev, uint64_t grad16_off,
-                                                                  int has_grad16) {
-    const bool skip = (found_inf != nullptr && *found_inf != 0);  // caller guarantees identical on all ranks
+                                                                  int has_grad16, uint64_t scaler_off) {
+    bool skip = !kScaler && (found_inf != nullptr && *found_inf != 0);  // caller guarantees identical on all ranks
+    float scale = scale_arg;
     __shared__ typename Rule::Cta cta;
     rule.prologue(cta, segs, lr_dev);                             // (the barrier below orders it for the whole CTA)
     // every rank's backward has finished writing its gradients
     if (!comm_block_barrier(c, 0, blockIdx.x)) return;
+    sod_loss_scaler* scaler = nullptr;
+    if constexpr (kScaler) {
+        __shared__ bool s_skip;
+        scaler = reinterpret_cast<sod_loss_scaler*>(c.peer[c.rank] + scaler_off);
+        if (threadIdx.x == 0) {
+            uint32_t any = 0u;
+            for (int q = 0; q < c.world; ++q)
+                any |= ld_acquire_sys(reinterpret_cast<const uint32_t*>(c.peer[q] + scaler_off));  // found_inf is word 0
+            s_skip = any != 0u;
+        }
+        __syncthreads();
+        skip = s_skip;
+        scale = (1.0f / scaler->scale) / static_cast<float>(c.world);
+    }
 
     const long long shard = (nvec + c.world - 1) / c.world;
     const long long stride = static_cast<long long>(gridDim.x) * kThreads;
@@ -432,7 +578,7 @@ __global__ void __launch_bounds__(kThreads) allreduce_step_kernel(const __grid_c
                 if (i < hi && cur.find(segs, i)) {        // frozen ranges and gaps are never consumed: not even reduced
                     sidx[u] = cur.s;
                     if (has_grad16 && (segs.flags[cur.s] & SOD_SEG_GRAD16))
-                        gv[u] = reduce_vec16(c, grad16_off + static_cast<uint64_t>(i) * 8u);
+                        gv[u] = reduce_vec16<H>(c, grad16_off + static_cast<uint64_t>(i) * 8u);
                     else
                         gv[u] = reduce_vec<kMulticast>(c, grad_off + static_cast<uint64_t>(i) * 16u);
                 }
@@ -474,11 +620,14 @@ __global__ void __launch_bounds__(kThreads) allreduce_step_kernel(const __grid_c
                     if (!only16) g_local[i] = zero;
                     if (g16_local != nullptr) g16_local[i] = make_uint2(0u, 0u);
                 }
-                if (shadow != nullptr && !skip) shadow[i] = f32x4_to_bf16(p_local[i]);
+                if (shadow != nullptr && !skip) shadow[i] = H::from_f32(p_local[i]);
             }
         }
     }
     rule.epilogue(segs, skip);
+    // every CTA of this rank has passed the end barrier, so every peer has read this rank's found_inf: the last CTA may
+    // overwrite it with the verdict
+    if constexpr (kScaler) scaler_epilogue(scaler, skip);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -558,9 +707,12 @@ static bool any_nesterov(const sod_sgd_segment* segs, int nseg) {
 }
 
 // world 1: validation shared by sod_sgd_momentum and sod_adam, then one streaming launch of local_step_kernel<Rule>
+// world 1: validation shared by sod_sgd_momentum, sod_adam and their *_scaler forms, then one streaming launch of
+// local_step_kernel<Rule, 16-bit format, scaler?>
 template <class Rule, class Seg>
 int launch_local_step(float* param, const Rule& rule, float* grad, void* grad16, void* shadow16, int64_t n, const Seg* segs,
-                      int nseg, const float* lr_dev, float inv_scale, const uint32_t* found_inf, int flags, void* stream) {
+                      int nseg, const float* lr_dev, float inv_scale, const uint32_t* found_inf, sod_loss_scaler* scaler,
+                      int flags, void* stream) {
     SOD_CHECK_ARG(param && grad && n > 0, SOD_EINVAL);
     SOD_CHECK_ARG((n & 3) == 0 && aligned16(param) && aligned16(grad), SOD_EALIGN);
     SOD_CHECK_ARG((!grad16 || aligned16(grad16)) && (!shadow16 || aligned16(shadow16)), SOD_EALIGN);
@@ -571,18 +723,24 @@ int launch_local_step(float* param, const Rule& rule, float* grad, void* grad16,
     long long blocks = (nvec + static_cast<long long>(kThreads) * kUnroll - 1) / (static_cast<long long>(kThreads) * kUnroll);
     const long long cap = 2ll * dev_info().sm_count;
     if (blocks > cap) blocks = cap;
-    local_step_kernel<Rule><<<static_cast<unsigned>(blocks), kThreads, 0, static_cast<cudaStream_t>(stream)>>>(
-        reinterpret_cast<float4*>(param), rule, reinterpret_cast<float4*>(grad),
-        reinterpret_cast<uint2*>(grad16), reinterpret_cast<uint2*>(shadow16), nvec, t, inv_scale, found_inf,
-        (flags & SOD_SGD_ZERO_GRAD) ? 1 : 0, lr_dev);
-    return static_cast<int>(cudaGetLastError());
+    auto go = [&](auto kernel) {
+        kernel<<<static_cast<unsigned>(blocks), kThreads, 0, static_cast<cudaStream_t>(stream)>>>(
+            reinterpret_cast<float4*>(param), rule, reinterpret_cast<float4*>(grad),
+            reinterpret_cast<uint2*>(grad16), reinterpret_cast<uint2*>(shadow16), nvec, t, inv_scale, found_inf,
+            (flags & SOD_SGD_ZERO_GRAD) ? 1 : 0, lr_dev, scaler);
+        return static_cast<int>(cudaGetLastError());
+    };
+    if (flags & SOD_GRAD16_F16)
+        return scaler ? go(local_step_kernel<Rule, F16x4, true>) : go(local_step_kernel<Rule, F16x4, false>);
+    return scaler ? go(local_step_kernel<Rule, Bf16x4, true>) : go(local_step_kernel<Rule, Bf16x4, false>);
 }
 
-// world > 1: validation shared by sod_allreduce_sgd and sod_allreduce_adam, then allreduce_step_kernel<Rule, multicast?>
+// world > 1: validation shared by sod_allreduce_sgd, sod_allreduce_adam and their *_scaler forms, then
+// allreduce_step_kernel<Rule, multicast?, 16-bit format, scaler?>
 template <class Rule, class Seg>
 int launch_allreduce_step(const sod_comm* comm, uint64_t grad_off, uint64_t grad16_off, uint64_t param_off, const Rule& rule,
                           void* shadow16, int64_t n, const Seg* segs, int nseg, const float* lr_dev, float inv_scale,
-                          const uint32_t* found_inf, int flags, void* stream) {
+                          const uint32_t* found_inf, sod_loss_scaler* scaler, int flags, void* stream) {
     SOD_CHECK_ARG(comm && n > 0, SOD_EINVAL);
     SOD_CHECK_ARG((n & 3) == 0 && (grad_off & 15) == 0 && (param_off & 15) == 0, SOD_EALIGN);
     CommDev c;
@@ -596,6 +754,13 @@ int launch_allreduce_step(const sod_comm* comm, uint64_t grad_off, uint64_t grad
         SOD_CHECK_ARG((grad16_off & 15) == 0, SOD_EALIGN);
         SOD_CHECK_ARG(grad16_off >= sod_comm_flag_bytes() && grad16_off + static_cast<uint64_t>(n) * 2 <= comm->arena_bytes, SOD_ECOMM);
     }
+    uint64_t scaler_off = 0;
+    if (scaler != nullptr) {   // the local scaler must be the arena's: its offset addresses every rank's copy
+        const uint64_t a = reinterpret_cast<uint64_t>(scaler), base = comm->peer[comm->rank];
+        SOD_CHECK_ARG((a & 15) == 0, SOD_EALIGN);
+        SOD_CHECK_ARG(a >= base + sod_comm_flag_bytes() && a + sizeof(sod_loss_scaler) <= base + comm->arena_bytes, SOD_ECOMM);
+        scaler_off = a - base;
+    }
     SegTable t;
     rc = make_seg_table(segs, nseg, n, t);
     if (rc != SOD_OK) return rc;
@@ -607,13 +772,19 @@ int launch_allreduce_step(const sod_comm* comm, uint64_t grad_off, uint64_t grad
     // NVLS wins (an all-reduce sweep, `bench.py --sweep`, decides this per system)
     const bool mc = (c.mc != 0) && !(flags & SOD_ALGO_NO_MULTIMEM) && (c.world > 2 || (flags & SOD_ALGO_FORCE_MULTIMEM));
     cudaStream_t s = static_cast<cudaStream_t>(stream);
-    if (mc)
-        allreduce_step_kernel<Rule, true><<<grid, kThreads, 0, s>>>(c, grad_off, param_off, rule, nvec, t, scale, found_inf, zg,
-                                                                    reinterpret_cast<uint2*>(shadow16), lr_dev, grad16_off, has16);
-    else
-        allreduce_step_kernel<Rule, false><<<grid, kThreads, 0, s>>>(c, grad_off, param_off, rule, nvec, t, scale, found_inf, zg,
-                                                                     reinterpret_cast<uint2*>(shadow16), lr_dev, grad16_off, has16);
-    return static_cast<int>(cudaGetLastError());
+    auto go = [&](auto kernel) {
+        kernel<<<grid, kThreads, 0, s>>>(c, grad_off, param_off, rule, nvec, t, scale, found_inf, zg,
+                                         reinterpret_cast<uint2*>(shadow16), lr_dev, grad16_off, has16, scaler_off);
+        return static_cast<int>(cudaGetLastError());
+    };
+    auto pick = [&](auto h, auto sc) {
+        using H = decltype(h);
+        constexpr bool kSc = decltype(sc)::value;
+        return mc ? go(allreduce_step_kernel<Rule, true, H, kSc>) : go(allreduce_step_kernel<Rule, false, H, kSc>);
+    };
+    if (flags & SOD_GRAD16_F16)
+        return scaler ? pick(F16x4{}, std::true_type{}) : pick(F16x4{}, std::false_type{});
+    return scaler ? pick(Bf16x4{}, std::true_type{}) : pick(Bf16x4{}, std::false_type{});
 }
 
 }  // namespace
@@ -627,9 +798,9 @@ extern "C" int sod_sgd_momentum(float* param, float* mom, float* grad, void* gra
     SOD_CHECK_ARG(aligned16(mom), SOD_EALIGN);
     if (any_nesterov(segs, nseg))
         return launch_local_step(param, SgdRule<true>{reinterpret_cast<float4*>(mom)}, grad, grad16, shadow16, n, segs, nseg,
-                                 lr_dev, inv_scale, found_inf, flags, stream);
+                                 lr_dev, inv_scale, found_inf, nullptr, flags, stream);
     return launch_local_step(param, SgdRule<false>{reinterpret_cast<float4*>(mom)}, grad, grad16, shadow16, n, segs, nseg,
-                             lr_dev, inv_scale, found_inf, flags, stream);
+                             lr_dev, inv_scale, found_inf, nullptr, flags, stream);
 }
 
 extern "C" int sod_adam(float* param, float* exp_avg, float* exp_avg_sq, float* grad, void* grad16, void* shadow16, int64_t n,
@@ -639,11 +810,14 @@ extern "C" int sod_adam(float* param, float* exp_avg, float* exp_avg_sq, float* 
     SOD_CHECK_ARG(param && exp_avg && exp_avg_sq && step_dev && grad && n > 0, SOD_EINVAL);
     SOD_CHECK_ARG(aligned16(exp_avg) && aligned16(exp_avg_sq), SOD_EALIGN);
     const AdamRule rule{reinterpret_cast<float4*>(exp_avg), reinterpret_cast<float4*>(exp_avg_sq), step_dev};
-    return launch_local_step(param, rule, grad, grad16, shadow16, n, segs, nseg, lr_dev, inv_scale, found_inf, flags, stream);
+    return launch_local_step(param, rule, grad, grad16, shadow16, n, segs, nseg, lr_dev, inv_scale, found_inf, nullptr, flags, stream);
 }
 
-extern "C" int sod_grad_gather16(const sod_gather_item* items, int nitems, void* dst16, int64_t dst_elems, void* stream) {
-    using namespace sod;
+namespace sod {
+namespace {
+
+template <uint32_t kExp>
+int gather16(const sod_gather_item* items, int nitems, void* dst16, int64_t dst_elems, uint32_t* found, void* stream) {
     SOD_CHECK_ARG(nitems >= 0 && (nitems == 0 || items) && dst16 && dst_elems > 0, SOD_EINVAL);
     SOD_CHECK_ARG(aligned16(dst16), SOD_EALIGN);
     for (int base = 0; base < nitems; base += kGatherMax) {
@@ -667,11 +841,38 @@ extern "C" int sod_grad_gather16(const sod_gather_item* items, int nitems, void*
         unsigned grid = chunks;
         const unsigned cap = 8u * static_cast<unsigned>(dev_info().sm_count);
         if (grid > cap) grid = cap;
-        grad_gather16_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(t, reinterpret_cast<uint4*>(dst16));
+        grad_gather16_kernel<kExp><<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(t, reinterpret_cast<uint4*>(dst16), found);
         const cudaError_t e = cudaGetLastError();
         if (e != cudaSuccess) return static_cast<int>(e);
     }
     return SOD_OK;
+}
+
+template <class H>
+int merge16(float* grad, void* grad16, int64_t n, void* stream) {
+    SOD_CHECK_ARG(grad && grad16 && n > 0, SOD_EINVAL);
+    SOD_CHECK_ARG((n & 3) == 0 && aligned16(grad) && aligned16(grad16), SOD_EALIGN);
+    const long long nvec = n >> 2;
+    long long blocks = (nvec + 1023) / 1024;
+    if (blocks > 8ll * dev_info().sm_count) blocks = 8ll * dev_info().sm_count;
+    grad_merge16_kernel<H><<<static_cast<unsigned>(blocks), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+        reinterpret_cast<float4*>(grad), reinterpret_cast<uint2*>(grad16), nvec);
+    return static_cast<int>(cudaGetLastError());
+}
+
+}  // namespace
+}  // namespace sod
+
+extern "C" int sod_grad_gather16(const sod_gather_item* items, int nitems, void* dst16, int64_t dst_elems, void* stream) {
+    return sod::gather16<0u>(items, nitems, dst16, dst_elems, nullptr, stream);
+}
+
+extern "C" int sod_grad_gather16_checked(const sod_gather_item* items, int nitems, void* dst16, int64_t dst_elems, int dtype,
+                                         uint32_t* found_inf, void* stream) {
+    using namespace sod;
+    SOD_CHECK_ARG(found_inf && (dtype == SOD_BF16 || dtype == SOD_F16), SOD_EINVAL);
+    return dtype == SOD_F16 ? gather16<F16x4::kExp>(items, nitems, dst16, dst_elems, found_inf, stream)
+                            : gather16<Bf16x4::kExp>(items, nitems, dst16, dst_elems, found_inf, stream);
 }
 
 extern "C" int sod_grad_nonfinite(const float* grad, int64_t n, uint32_t* found_inf, void* stream) {
@@ -686,16 +887,51 @@ extern "C" int sod_grad_nonfinite(const float* grad, int64_t n, uint32_t* found_
     return static_cast<int>(cudaGetLastError());
 }
 
-extern "C" int sod_grad_merge_bf16(float* grad, void* grad16, int64_t n, void* stream) {
+extern "C" int sod_grad_check_ranges(const float* grad, const void* grad16, int64_t n, const sod_check_range* ranges,
+                                     int nranges, int flags, uint32_t* found_inf, void* stream) {
     using namespace sod;
-    SOD_CHECK_ARG(grad && grad16 && n > 0, SOD_EINVAL);
-    SOD_CHECK_ARG((n & 3) == 0 && aligned16(grad) && aligned16(grad16), SOD_EALIGN);
-    const long long nvec = n >> 2;
-    long long blocks = (nvec + 1023) / 1024;
-    if (blocks > 8ll * dev_info().sm_count) blocks = 8ll * dev_info().sm_count;
-    grad_merge_bf16_kernel<<<static_cast<unsigned>(blocks), 256, 0, static_cast<cudaStream_t>(stream)>>>(
-        reinterpret_cast<float4*>(grad), reinterpret_cast<uint2*>(grad16), nvec);
-    return static_cast<int>(cudaGetLastError());
+    SOD_CHECK_ARG(found_inf && n > 0 && nranges >= 0 && (nranges == 0 || ranges), SOD_EINVAL);
+    for (int base = 0; base < nranges; base += kCheckMax) {
+        CheckTable t;
+        t.n = 0;
+        unsigned chunks = 0;
+        for (int i = base; i < nranges && i < base + kCheckMax; ++i) {
+            const sod_check_range& r = ranges[i];
+            const bool in16 = (r.flags & SOD_SEG_GRAD16) != 0;
+            if (r.begin < 0 || r.end < r.begin || r.end > n || r.end - r.begin > 0x7fffffffll) return SOD_EINVAL;
+            if (in16 ? grad16 == nullptr : grad == nullptr) return SOD_EINVAL;
+            if (r.end == r.begin) continue;
+            t.begin[t.n] = r.begin;
+            t.numel[t.n] = static_cast<unsigned>(r.end - r.begin);
+            t.in16[t.n] = in16 ? 1 : 0;
+            t.chunk0[t.n] = chunks;
+            chunks += static_cast<unsigned>((r.end - r.begin + kCheckChunk - 1) / kCheckChunk);
+            ++t.n;
+        }
+        t.chunk0[t.n] = chunks;
+        if (chunks == 0) continue;
+        unsigned grid = chunks;
+        const unsigned cap = 4u * static_cast<unsigned>(dev_info().sm_count);
+        if (grid > cap) grid = cap;
+        cudaStream_t s = static_cast<cudaStream_t>(stream);
+        const unsigned short* g16 = static_cast<const unsigned short*>(grad16);
+        if (flags & SOD_GRAD16_F16)
+            grad_check_ranges_kernel<F16x4::kExp><<<grid, 256, 0, s>>>(t, grad, g16, found_inf);
+        else
+            grad_check_ranges_kernel<Bf16x4::kExp><<<grid, 256, 0, s>>>(t, grad, g16, found_inf);
+        const cudaError_t e = cudaGetLastError();
+        if (e != cudaSuccess) return static_cast<int>(e);
+    }
+    return SOD_OK;
+}
+
+extern "C" int sod_grad_merge_bf16(float* grad, void* grad16, int64_t n, void* stream) {
+    return sod::merge16<sod::Bf16x4>(grad, grad16, n, stream);
+}
+
+extern "C" int sod_grad_merge16(float* grad, void* grad16, int64_t n, int flags, void* stream) {
+    return (flags & SOD_GRAD16_F16) ? sod::merge16<sod::F16x4>(grad, grad16, n, stream)
+                                    : sod::merge16<sod::Bf16x4>(grad, grad16, n, stream);
 }
 
 extern "C" int sod_allreduce_sgd(const sod_comm* comm, uint64_t grad_off, uint64_t grad16_off, uint64_t param_off, float* mom,
@@ -706,9 +942,9 @@ extern "C" int sod_allreduce_sgd(const sod_comm* comm, uint64_t grad_off, uint64
     SOD_CHECK_ARG(aligned16(mom), SOD_EALIGN);
     if (any_nesterov(segs, nseg))
         return launch_allreduce_step(comm, grad_off, grad16_off, param_off, SgdRule<true>{reinterpret_cast<float4*>(mom)},
-                                     shadow16, n, segs, nseg, lr_dev, inv_scale, found_inf, flags, stream);
+                                     shadow16, n, segs, nseg, lr_dev, inv_scale, found_inf, nullptr, flags, stream);
     return launch_allreduce_step(comm, grad_off, grad16_off, param_off, SgdRule<false>{reinterpret_cast<float4*>(mom)},
-                                 shadow16, n, segs, nseg, lr_dev, inv_scale, found_inf, flags, stream);
+                                 shadow16, n, segs, nseg, lr_dev, inv_scale, found_inf, nullptr, flags, stream);
 }
 
 extern "C" int sod_allreduce_adam(const sod_comm* comm, uint64_t grad_off, uint64_t grad16_off, uint64_t param_off,
@@ -720,7 +956,55 @@ extern "C" int sod_allreduce_adam(const sod_comm* comm, uint64_t grad_off, uint6
     SOD_CHECK_ARG(aligned16(exp_avg) && aligned16(exp_avg_sq), SOD_EALIGN);
     const AdamRule rule{reinterpret_cast<float4*>(exp_avg), reinterpret_cast<float4*>(exp_avg_sq), step_dev};
     return launch_allreduce_step(comm, grad_off, grad16_off, param_off, rule, shadow16, n, segs, nseg, lr_dev, inv_scale,
-                                 found_inf, flags, stream);
+                                 found_inf, nullptr, flags, stream);
+}
+
+extern "C" int sod_sgd_momentum_scaler(float* param, float* mom, float* grad, void* grad16, void* shadow16, int64_t n,
+                                       const sod_sgd_segment* segs, int nseg, const float* lr_dev, sod_loss_scaler* scaler,
+                                       int flags, void* stream) {
+    using namespace sod;
+    SOD_CHECK_ARG(param && mom && grad && scaler && n > 0, SOD_EINVAL);
+    SOD_CHECK_ARG(aligned16(mom), SOD_EALIGN);
+    if (any_nesterov(segs, nseg))
+        return launch_local_step(param, SgdRule<true>{reinterpret_cast<float4*>(mom)}, grad, grad16, shadow16, n, segs, nseg,
+                                 lr_dev, 1.0f, nullptr, scaler, flags, stream);
+    return launch_local_step(param, SgdRule<false>{reinterpret_cast<float4*>(mom)}, grad, grad16, shadow16, n, segs, nseg,
+                             lr_dev, 1.0f, nullptr, scaler, flags, stream);
+}
+
+extern "C" int sod_adam_scaler(float* param, float* exp_avg, float* exp_avg_sq, float* grad, void* grad16, void* shadow16,
+                               int64_t n, const sod_adam_segment* segs, int nseg, const float* lr_dev, int32_t* step_dev,
+                               sod_loss_scaler* scaler, int flags, void* stream) {
+    using namespace sod;
+    SOD_CHECK_ARG(param && exp_avg && exp_avg_sq && step_dev && grad && scaler && n > 0, SOD_EINVAL);
+    SOD_CHECK_ARG(aligned16(exp_avg) && aligned16(exp_avg_sq), SOD_EALIGN);
+    const AdamRule rule{reinterpret_cast<float4*>(exp_avg), reinterpret_cast<float4*>(exp_avg_sq), step_dev};
+    return launch_local_step(param, rule, grad, grad16, shadow16, n, segs, nseg, lr_dev, 1.0f, nullptr, scaler, flags, stream);
+}
+
+extern "C" int sod_allreduce_sgd_scaler(const sod_comm* comm, uint64_t grad_off, uint64_t grad16_off, uint64_t param_off,
+                                        float* mom, void* shadow16, int64_t n, const sod_sgd_segment* segs, int nseg,
+                                        const float* lr_dev, sod_loss_scaler* scaler, int flags, void* stream) {
+    using namespace sod;
+    SOD_CHECK_ARG(comm && mom && scaler && n > 0, SOD_EINVAL);
+    SOD_CHECK_ARG(aligned16(mom), SOD_EALIGN);
+    if (any_nesterov(segs, nseg))
+        return launch_allreduce_step(comm, grad_off, grad16_off, param_off, SgdRule<true>{reinterpret_cast<float4*>(mom)},
+                                     shadow16, n, segs, nseg, lr_dev, 1.0f, nullptr, scaler, flags, stream);
+    return launch_allreduce_step(comm, grad_off, grad16_off, param_off, SgdRule<false>{reinterpret_cast<float4*>(mom)},
+                                 shadow16, n, segs, nseg, lr_dev, 1.0f, nullptr, scaler, flags, stream);
+}
+
+extern "C" int sod_allreduce_adam_scaler(const sod_comm* comm, uint64_t grad_off, uint64_t grad16_off, uint64_t param_off,
+                                         float* exp_avg, float* exp_avg_sq, void* shadow16, int64_t n,
+                                         const sod_adam_segment* segs, int nseg, const float* lr_dev, int32_t* step_dev,
+                                         sod_loss_scaler* scaler, int flags, void* stream) {
+    using namespace sod;
+    SOD_CHECK_ARG(comm && exp_avg && exp_avg_sq && step_dev && scaler && n > 0, SOD_EINVAL);
+    SOD_CHECK_ARG(aligned16(exp_avg) && aligned16(exp_avg_sq), SOD_EALIGN);
+    const AdamRule rule{reinterpret_cast<float4*>(exp_avg), reinterpret_cast<float4*>(exp_avg_sq), step_dev};
+    return launch_allreduce_step(comm, grad_off, grad16_off, param_off, rule, shadow16, n, segs, nseg, lr_dev, 1.0f, nullptr,
+                                 scaler, flags, stream);
 }
 
 extern "C" int sod_allreduce_f32(const sod_comm* comm, uint64_t off, int64_t n, float scale, int algo, int flags,

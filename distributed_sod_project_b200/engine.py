@@ -62,8 +62,10 @@ class Trainer:
         # CUDA-graph replay of the whole iteration (SURVEY §8f.1): one cudaGraphLaunch instead of ~1500 launches.
         # One graph per input shape (multi-scale training, reference utils/dataset.py:125-132, cycles through three);
         # learning rates are read from a device table (FusedOptimizer.sync_lr), so the scheduler never forces a re-capture.
+        # fp16's dynamic loss scale lives on the device (amp.py), so it replays too.
         from .optim import FusedOptimizer
-        self.use_graph = use_graph and not amp._cfg["dynamic"] and isinstance(self.optimizer, FusedOptimizer)
+        self.use_graph = use_graph and isinstance(self.optimizer, FusedOptimizer) and \
+            (not amp._cfg["dynamic"] or self.optimizer.flat.scaler is not None)
         self._graphs: dict = {}
         self._cur = None
 
@@ -84,14 +86,19 @@ class Trainer:
     def _iteration(self, x: torch.Tensor, m: torch.Tensor, report: bool):
         if self.channels_last:
             x = x.contiguous(memory_format=torch.channels_last)
+        amp.push()                                                         # host writes of the loss scale (fp16)
         preds = self.model(x)                                              # train.py:293
         unit = not amp._cfg["dynamic"]
+        # fp16: the fused loss forms its gradient already multiplied by the device loss scale; scale_loss multiplies the
+        # loss by the same tensor, so backward hands that gradient on untouched
+        sdev = amp.scale_tensor() if self.use_amp and amp._cfg["dynamic"] else None
+        extra = (sdev,) if sdev is not None else ()
         if len(self.loss_funcs) == 2 and not report:
             holder: list = []
-            loss = _FusedLossFn.apply(preds, m, self.loss_funcs[0].reduction, 1.0, 1.0, 1e-6, unit, 0, holder)
+            loss = _FusedLossFn.apply(preds, m, self.loss_funcs[0].reduction, 1.0, 1.0, 1e-6, unit, 0, holder, *extra)
             items = holder[0]                                              # device scalars [bce, cel, total, ...]
         else:
-            loss, items = get_total_loss(preds, m, self.loss_funcs, unit_upstream=unit)   # train.py:295
+            loss, items = get_total_loss(preds, m, self.loss_funcs, unit_upstream=unit, scale_dev=sdev)   # train.py:295
         self.optimizer.zero_grad()                                         # train.py:297
         if self.use_amp:
             with amp.scale_loss(loss, self.optimizer) as scaled:           # train.py:299
@@ -105,8 +112,9 @@ class Trainer:
     def _capture(self, x: torch.Tensor, m: torch.Tensor) -> dict:
         """warm up eagerly on a side stream, then record one whole iteration into a CUDA graph"""
         static_x, static_m = x.clone(), m.clone()
+        amp.push()                                   # a pending host write of the loss scale belongs to the state kept
         # the warm-up iterations (allocator, cuDNN autotune, autograd thread) must not move the training state
-        snap = self.optimizer.snapshot()             # parameters, optimizer state (Adam: its step counts), shadow
+        snap = self.optimizer.snapshot()             # parameters, optimizer state (Adam: its step counts), shadow, scaler
         buffers = [b.clone() for b in self.module.buffers()]
         side = torch.cuda.Stream()
         side.wait_stream(torch.cuda.current_stream())
@@ -115,6 +123,8 @@ class Trainer:
                 self._iteration(static_x, static_m, report=False)
         torch.cuda.current_stream().wait_stream(side)
         self.optimizer.restore(snap)
+        if amp._cfg["dynamic"]:
+            amp.read_scaler()                        # the host mirror back to the restored scaler
         with torch.no_grad():
             for b, old in zip(self.module.buffers(), buffers):
                 b.copy_(old)
@@ -144,6 +154,7 @@ class Trainer:
 
     def _replay(self, ent: dict) -> None:
         self.optimizer.sync_lr()                              # param_groups[i]["lr"] → device table, only when it moved
+        amp.push()                                            # host writes of the fp16 loss scale, only when there are any
         ent["graph"].replay()
         self.optimizer.steps += 1
         self.optimizer._stepped = True

@@ -30,9 +30,11 @@ def _workspace(device: torch.device) -> torch.Tensor:
 
 
 def bce_cel_fwd_bwd(logits: torch.Tensor, mask: torch.Tensor, *, reduction: str = "mean", w_bce: float = 1.0,
-                    w_cel: float = 1.0, grad_scale: float = 1.0, eps: float = 1e-6, mode: int = 0):
+                    w_cel: float = 1.0, grad_scale: float = 1.0, eps: float = 1e-6, mode: int = 0,
+                    grad_scale_dev: torch.Tensor | None = None):
     """Raw call into `sod_loss_bce_cel_fwd_bwd`. Returns (scalars[8] fp32 device tensor, grad like logits).
-    scalars = [bce, cel, total, Σp, Σt, Σp·t, bce_sum, n]."""
+    scalars = [bce, cel, total, Σp, Σt, Σp·t, bce_sum, n].  grad_scale_dev (fp32 device scalar, e.g. the amp loss scale):
+    the gradient is multiplied by it before it is rounded to the logits dtype (`sod_loss_bce_cel_fwd_bwd_scaled`)."""
     if not logits.is_cuda:
         raise _lib.SodError("the fused BCE+CEL loss runs on CUDA tensors only (no CPU fallback)")
     if reduction not in ("mean", "sum"):
@@ -51,6 +53,17 @@ def bce_cel_fwd_bwd(logits: torch.Tensor, mask: torch.Tensor, *, reduction: str 
     grad = torch.empty_like(x)
     scalars = torch.empty(8, dtype=torch.float32, device=x.device)
     ws = _workspace(x.device)
+    if grad_scale_dev is not None:
+        if grad_scale_dev.dtype != torch.float32 or grad_scale_dev.numel() != 1 or grad_scale_dev.device != x.device:
+            raise _lib.SodError("grad_scale_dev must be one fp32 element on the logits' device")
+        rc = _lib.lib().sod_loss_bce_cel_fwd_bwd_scaled(
+            x.data_ptr(), _lib.dtype_code(x.dtype), m.data_ptr(), _lib.dtype_code(m.dtype), grad.data_ptr(),
+            _lib.dtype_code(x.dtype), scalars.data_ptr(), x.numel(), 1 if reduction == "sum" else 0,
+            float(w_bce), float(w_cel), float(grad_scale), grad_scale_dev.data_ptr(), float(eps), int(mode), ws.data_ptr(),
+            ws.numel(), _lib.stream_ptr())
+        _lib.check(rc, "sod_loss_bce_cel_fwd_bwd_scaled")
+        _lib.count_launch()
+        return scalars, grad
     rc = _lib.lib().sod_loss_bce_cel_fwd_bwd(
         x.data_ptr(), _lib.dtype_code(x.dtype), m.data_ptr(), _lib.dtype_code(m.dtype), grad.data_ptr(),
         _lib.dtype_code(x.dtype), scalars.data_ptr(), x.numel(), 1 if reduction == "sum" else 0,
@@ -62,11 +75,20 @@ def bce_cel_fwd_bwd(logits: torch.Tensor, mask: torch.Tensor, *, reduction: str 
 
 
 class _FusedLossFn(torch.autograd.Function):
+    """apply(logits, mask, reduction, w_bce, w_cel, eps, unit_upstream, mode, holder[, scale_dev]).
+
+    scale_dev (optional, fp32 0-d device tensor — the amp loss scale): the gradient is formed as scale_dev × d total/d logits
+    and rounded once, and backward hands it to autograd untouched.  Contract: `.backward()` is called on
+    `total * scale_dev` with that same tensor (what `amp.scale_loss` yields), so the upstream gradient IS scale_dev."""
+
     @staticmethod
-    def forward(ctx, logits, mask, reduction, w_bce, w_cel, eps, unit_upstream, mode, holder):
-        scalars, grad = bce_cel_fwd_bwd(logits, mask, reduction=reduction, w_bce=w_bce, w_cel=w_cel, eps=eps, mode=mode)
+    def forward(ctx, logits, mask, reduction, w_bce, w_cel, eps, unit_upstream, mode, holder, *scale_dev):
+        sdev = scale_dev[0] if scale_dev else None
+        scalars, grad = bce_cel_fwd_bwd(logits, mask, reduction=reduction, w_bce=w_bce, w_cel=w_cel, eps=eps, mode=mode,
+                                        grad_scale_dev=sdev)
         ctx.save_for_backward(grad)
-        ctx.unit_upstream = unit_upstream
+        ctx.unit_upstream = unit_upstream or sdev is not None
+        ctx.n_extra = len(scale_dev)
         holder.append(scalars)          # side channel: the 8 report scalars, no extra kernel
         return scalars[2]               # 0-d view of the kernel's output buffer
 
@@ -80,7 +102,7 @@ class _FusedLossFn(torch.autograd.Function):
                                                        g.data_ptr(), _lib.stream_ptr())
             _lib.check(rc, "sod_scale_by_device_scalar")
             _lib.count_launch()
-        return grad, None, None, None, None, None, None, None, None
+        return (grad,) + (None,) * (8 + ctx.n_extra)
 
 
 class FusedBCECEL(nn.Module):
@@ -135,14 +157,16 @@ def _as_pair(loss_funcs):
 
 
 def get_total_loss(train_preds: torch.Tensor, train_masks: torch.Tensor, loss_funcs: list,
-                   unit_upstream: bool = False):
-    """Signature and return contract of reference utils/pipeline_ops.py:19-43."""
+                   unit_upstream: bool = False, scale_dev: torch.Tensor | None = None):
+    """Signature and return contract of reference utils/pipeline_ops.py:19-43.  scale_dev: the amp loss scale the fused
+    pair's gradient is formed with (see `_FusedLossFn`); backward must then run on `total * scale_dev`."""
     assert len(loss_funcs) != 0, "请指定损失函数`loss_funcs`"
     pair = _as_pair(loss_funcs) if train_preds.is_cuda else None
     if pair is not None:
         reduction, eps = pair
         holder: list = []
-        total = _FusedLossFn.apply(train_preds, train_masks, reduction, 1.0, 1.0, eps, unit_upstream, 0, holder)
+        extra = (scale_dev,) if scale_dev is not None else ()
+        total = _FusedLossFn.apply(train_preds, train_masks, reduction, 1.0, 1.0, eps, unit_upstream, 0, holder, *extra)
         host = holder[0][:2].tolist()          # one 8-byte D2H + one sync for both report strings
         return total, [f"{host[0]:.5f}", f"{host[1]:.5f}"]
     loss_list, items = [], []

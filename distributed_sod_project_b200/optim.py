@@ -69,8 +69,12 @@ class FlatParams:
         self.mom = torch.zeros(off, dtype=torch.float32, device=dev)
         self.arena = None          # set by DistributedDataParallel when world > 1
         self.param_off = self.grad_off = self.grad16_off = 0
-        self.shadow16: torch.Tensor | None = None   # bf16 copy of `param`, refreshed by the fused step (amp O1 shadow)
-        self.grad16: torch.Tensor | None = None     # bf16 gradients autograd accumulates for the shadowed tensors
+        self.shadow16: torch.Tensor | None = None   # bf16/fp16 copy of `param`, refreshed by the fused step (amp O1 shadow)
+        self.grad16: torch.Tensor | None = None     # 16-bit gradients (the shadow's dtype) autograd makes for the shadowed tensors
+        # amp fp16: the device-resident loss scaler (`sod_loss_scaler`, int32 words; the scale is word 1 as fp32 bits), in
+        # the symmetric arena at scaler_off when world > 1
+        self.scaler: torch.Tensor | None = None
+        self.scaler_off = 0
         # bf16 shadow leaves the convolutions consume (amp._install_shadow_weights): (leaf, element offset, steal)
         # steal=True: `.grad` is left None so that autograd hands over cuDNN's gradient tensor as it is (no accumulate
         # kernel per parameter); the fused step collects all of them into `grad16` with one sod_grad_gather16 launch
@@ -80,14 +84,30 @@ class FlatParams:
         self.master_grads_seen = False
         self._bind(copy_from_params=True)
 
-    # -- mixed precision: bf16 shadow of the fp32 master ---------------------------------------------------
+    # -- mixed precision: 16-bit shadow of the fp32 master ---------------------------------------------------
     def enable_shadow(self, dtype: torch.dtype = torch.bfloat16) -> None:
-        if dtype != torch.bfloat16:
-            raise _lib.SodError("the shadow copy is bf16 (fp16 needs dynamic loss scaling: handled without a shadow)")
+        """bf16 (amp bf16) or fp16 (amp fp16, with the device loss scaler); `grad16` takes the same dtype"""
+        if dtype not in (torch.bfloat16, torch.float16):
+            raise _lib.SodError(f"the shadow copy is bf16 or fp16, not {dtype}")
+        if self.shadow16 is not None and self.shadow16.dtype != dtype:
+            raise _lib.SodError(f"the shadow copy is already {self.shadow16.dtype}")
         if self.shadow16 is None:
             self.shadow16 = torch.zeros(self.numel, dtype=dtype, device=self.device)
             self.grad16 = torch.zeros(self.numel, dtype=dtype, device=self.device)
         self.refresh_shadow()
+
+    def enable_scaler(self, scale: float, growth_interval: int) -> None:
+        """the device-resident dynamic loss scale of amp fp16 (include/sod_b200.h `sod_loss_scaler`)"""
+        if self.scaler is None:
+            self.scaler = torch.zeros(_lib.SOD_LOSS_SCALER_WORDS, dtype=torch.int32, device=self.device)
+        self.scaler.zero_()
+        self.scaler.view(torch.float32)[1].fill_(float(scale))
+        self.scaler[3].fill_(int(growth_interval))
+
+    @property
+    def flags16(self) -> int:
+        """the step kernels' flag for the 16-bit buffers' format"""
+        return _lib.SOD_GRAD16_F16 if self.grad16 is not None and self.grad16.dtype == torch.float16 else 0
 
     def refresh_shadow(self) -> None:
         if self.shadow16 is not None:
@@ -140,6 +160,12 @@ class FlatParams:
             for leaf, off, steal in self.shadow_leaves:
                 if not steal and leaf.requires_grad:
                     leaf.grad = self._view(self.grad16, off, leaf)
+        if self.scaler is not None:
+            # every rank's step kernel reads every rank's overflow flag: the scaler has to be peer-readable
+            self.scaler_off = arena.alloc(4 * _lib.SOD_LOSS_SCALER_WORDS)
+            new_s = arena.view(self.scaler_off, _lib.SOD_LOSS_SCALER_WORDS, torch.int32)
+            new_s.copy_(self.scaler)
+            self.scaler = new_s
         self.refresh_shadow()
 
     def momentum_view(self, p: nn.Parameter) -> torch.Tensor:
@@ -183,8 +209,9 @@ class FusedOptimizer(Optimizer):
         self.flat = FlatParams([list(g["params"]) for g in self.param_groups], leftovers, bf16_grad_ids=conv_ids)
         for p, _ in self.flat.slots:
             flat_registry[id(p)] = self.flat
-        self.inv_scale = 1.0                   # amp: 1/S for the coming step
-        self.found_inf: torch.Tensor | None = None  # amp: device uint32 flag, or None
+        self.inv_scale = 1.0                   # static loss scale: 1/S for the coming step
+        self._found_inf: torch.Tensor | None = None  # static loss scale: device uint32 flag, or None
+        self._scaler_readback = None           # amp fp16: refreshes amp's host mirror after an eager step
         self._grads_clean = True
         self._clean_version = self._grad_versions()
         self._stepped = False
@@ -204,11 +231,23 @@ class FusedOptimizer(Optimizer):
         """one entry of the kernels' segment table; g is None for the frozen parameters outside every group"""
         raise NotImplementedError
 
-    def _launch_local(self, segs, n, lr_dev, g16, s16, finf) -> None:
+    def _launch_local(self, segs, n, lr_dev, g16, s16, finf, scaler) -> None:
+        """scaler: address of the device loss scaler (then finf / inv_scale are not used), or None"""
         raise NotImplementedError
 
-    def _launch_allreduce(self, segs, n, lr_dev, g16, s16, finf) -> None:
+    def _launch_allreduce(self, segs, n, lr_dev, g16, s16, finf, scaler) -> None:
         raise NotImplementedError
+
+    @property
+    def found_inf(self) -> torch.Tensor | None:
+        """device uint32 overflow flag of the last step: with amp fp16 a view of the loss scaler's found_inf word"""
+        if self.flat.scaler is not None:
+            return self.flat.scaler[0:1]
+        return self._found_inf
+
+    @found_inf.setter
+    def found_inf(self, t: torch.Tensor | None) -> None:
+        self._found_inf = t
 
     # -------------------------------------------------------------------------------------------------------
     def _grad_versions(self):
@@ -278,12 +317,14 @@ class FusedOptimizer(Optimizer):
             elif leaf.grad is None or leaf.grad.data_ptr() != self.flat.grad16.data_ptr() + 2 * off:
                 leaf.grad = FlatParams._view(self.flat.grad16, off, leaf)
 
-    def _gather_stolen(self) -> None:
-        """bf16 gradients autograd left in their own tensors (shadow leaves with steal=True, or any leaf whose `.grad`
-        was replaced) → flat `grad16`, one launch for all of them"""
+    def _gather_stolen(self, finf: int | None = None) -> set:
+        """16-bit gradients autograd left in their own tensors (shadow leaves with steal=True, or any leaf whose `.grad`
+        was replaced) → flat `grad16`, one launch for all of them.  finf (amp fp16): address of the overflow flag the
+        gather ORs the non-finiteness of what it copies into.  Returns the offsets of the leaves it gathered."""
         f = self.flat
+        gathered = set()
         if not f.shadow_leaves:
-            return
+            return gathered
         base = f.grad16.data_ptr()
         items = []
         for leaf, off, _ in f.shadow_leaves:
@@ -292,6 +333,7 @@ class FusedOptimizer(Optimizer):
                 continue
             if g.dtype == f.grad16.dtype and g.is_cuda and g.numel() == leaf.numel() and _same_physical_order(g, leaf):
                 items.append((g.data_ptr(), off, g.numel()))
+                gathered.add(off)
             else:                                            # unusual layout / dtype: plain torch accumulate
                 FlatParams._view(f.grad16, off, leaf).add_(g.to(f.grad16.dtype))
         if items:
@@ -300,9 +342,43 @@ class FusedOptimizer(Optimizer):
                 self._gather_key = key
                 self._gather_arr = (_lib.sod_gather_item * len(items))(*[_lib.sod_gather_item(a, b, c) for a, b, c in items])
             arr = self._gather_arr
-            rc = _lib.lib().sod_grad_gather16(arr, len(items), base, f.numel, _lib.stream_ptr())
-            _lib.check(rc, "sod_grad_gather16")
+            if finf is None:
+                rc = _lib.lib().sod_grad_gather16(arr, len(items), base, f.numel, _lib.stream_ptr())
+                _lib.check(rc, "sod_grad_gather16")
+            else:
+                rc = _lib.lib().sod_grad_gather16_checked(arr, len(items), base, f.numel, _lib.dtype_code(f.grad16.dtype),
+                                                          finf, _lib.stream_ptr())
+                _lib.check(rc, "sod_grad_gather16_checked")
             _lib.count_launch((len(items) + _lib.SOD_GATHER_MAX_ITEMS - 1) // _lib.SOD_GATHER_MAX_ITEMS)
+        return gathered
+
+    def _check_rest(self, finf: int, gathered: set) -> None:
+        """amp fp16: OR into the flag the non-finiteness of every gradient the checked gather did not read — the fp32
+        gradients of the ranges without SOD_SEG_GRAD16 (BN γ/β, leftovers) and the 16-bit gradients accumulated in place
+        (folded convolution biases).  After a forward outside autocast (fp32 gradients for the convolution parameters
+        too) the whole fp32 buffer is read instead."""
+        f = self.flat
+        exclusive = self._bf16_exclusive()
+        ranges = [] if not exclusive else \
+            [(b, e, 0) for b, e, _, part16 in self._segment_plan() if not part16]
+        for leaf, off, _ in f.shadow_leaves:
+            if off not in gathered:
+                ranges.append((off, off + leaf.numel(), _lib.SOD_SEG_GRAD16))
+        if not exclusive:
+            rc = _lib.lib().sod_grad_nonfinite(f.grad.data_ptr(), f.numel, finf, _lib.stream_ptr())
+            _lib.check(rc, "sod_grad_nonfinite")
+            _lib.count_launch()
+        if not ranges:
+            return
+        key = tuple(ranges)
+        if getattr(self, "_check_key", None) != key:
+            self._check_key = key
+            self._check_arr = (_lib.sod_check_range * len(ranges))(*[_lib.sod_check_range(b, e, fl) for b, e, fl in ranges])
+        g16 = f.grad16.data_ptr() if f.grad16 is not None else None
+        rc = _lib.lib().sod_grad_check_ranges(f.grad.data_ptr(), g16, f.numel, self._check_arr, len(ranges), f.flags16, finf,
+                                              _lib.stream_ptr())
+        _lib.check(rc, "sod_grad_check_ranges")
+        _lib.count_launch((len(ranges) + _lib.SOD_CHECK_MAX_RANGES - 1) // _lib.SOD_CHECK_MAX_RANGES)
 
     def _segments(self):
         plan = self._segment_plan()
@@ -323,21 +399,34 @@ class FusedOptimizer(Optimizer):
         segs, n = self._segments()
         self.sync_lr()
         lr_dev = self._lr_dev.data_ptr()
-        self._gather_stolen()
-        finf = self.found_inf.data_ptr() if self.found_inf is not None else None
+        scaler = f.scaler.data_ptr() if f.scaler is not None else None
+        if scaler is not None:
+            # amp fp16: clear the flag (stream order puts this after the previous step, which every peer has left), then
+            # the checks: the gather checks what it copies, one small launch the rest; the step reads the verdict
+            f.scaler[0:1].zero_()
+            self._check_rest(scaler, self._gather_stolen(finf=scaler))
+            finf = None
+        else:
+            self._gather_stolen()
+            finf = self._found_inf.data_ptr() if self._found_inf is not None else None
         g16 = f.grad16.data_ptr() if f.grad16 is not None else None
         s16 = f.shadow16.data_ptr() if f.shadow16 is not None else None
         if f.arena is None:
-            self._launch_local(segs, n, lr_dev, g16, s16, finf)
+            self._launch_local(segs, n, lr_dev, g16, s16, finf, scaler)
         else:
             if g16 is not None and not self._bf16_exclusive():
                 # fp32 gradients were written for the convolution parameters too (model ran outside autocast): fold the
-                # bf16 ones into the fp32 symmetric buffer and exchange that
-                rc = _lib.lib().sod_grad_merge_bf16(f.grad.data_ptr(), g16, f.numel, _lib.stream_ptr())
-                _lib.check(rc, "sod_grad_merge_bf16")
+                # 16-bit ones into the fp32 symmetric buffer and exchange that
+                if f.flags16:
+                    rc = _lib.lib().sod_grad_merge16(f.grad.data_ptr(), g16, f.numel, f.flags16, _lib.stream_ptr())
+                else:
+                    rc = _lib.lib().sod_grad_merge_bf16(f.grad.data_ptr(), g16, f.numel, _lib.stream_ptr())
+                _lib.check(rc, "sod_grad_merge")
                 _lib.count_launch()
-            self._launch_allreduce(segs, n, lr_dev, g16, s16, finf)
+            self._launch_allreduce(segs, n, lr_dev, g16, s16, finf, scaler)
         _lib.count_launch()
+        if scaler is not None and self._scaler_readback is not None and not torch.cuda.is_current_stream_capturing():
+            self._scaler_readback()
         f.master_grads_seen = False
         self._grads_clean = True
         self._clean_version = self._grad_versions()
@@ -370,7 +459,8 @@ class FusedOptimizer(Optimizer):
 
     # -- CUDA-graph capture: the warm-up iterations must not move the training state ------------------------
     def snapshot(self) -> dict:
-        """copies of everything a step changes: parameters, optimizer state, the bf16 shadow, the step counts"""
+        """copies of everything a step changes: parameters, optimizer state, the 16-bit shadow, the step counts, the loss
+        scaler"""
         return dict(tensors=[t.clone() for t in self._snapshot_tensors()], steps=self.steps, stepped=self._stepped)
 
     @torch.no_grad()
@@ -381,7 +471,8 @@ class FusedOptimizer(Optimizer):
 
     def _snapshot_tensors(self) -> list[torch.Tensor]:
         f = self.flat
-        return [f.param, *self._state_buffers()] + ([f.shadow16] if f.shadow16 is not None else [])
+        return [f.param, *self._state_buffers()] + ([f.shadow16] if f.shadow16 is not None else []) + \
+            ([f.scaler] if f.scaler is not None else [])
 
 
 class FusedSGD(FusedOptimizer):
@@ -404,18 +495,27 @@ class FusedSGD(FusedOptimizer):
             flags |= _lib.SOD_SEG_NESTEROV
         return _lib.sod_sgd_segment(b, e, float(g["lr"]), float(g["weight_decay"]), float(g["momentum"]), flags)
 
-    def _launch_local(self, segs, n, lr_dev, g16, s16, finf):
+    def _launch_local(self, segs, n, lr_dev, g16, s16, finf, scaler=None):
         f = self.flat
-        rc = _lib.lib().sod_sgd_momentum(f.param.data_ptr(), f.mom.data_ptr(), f.grad.data_ptr(), g16, s16, f.numel,
-                                         segs, n, lr_dev, float(self.inv_scale), finf, _lib.SOD_SGD_ZERO_GRAD,
-                                         _lib.stream_ptr())
+        flags = _lib.SOD_SGD_ZERO_GRAD | f.flags16
+        if scaler is not None:
+            rc = _lib.lib().sod_sgd_momentum_scaler(f.param.data_ptr(), f.mom.data_ptr(), f.grad.data_ptr(), g16, s16, f.numel,
+                                                    segs, n, lr_dev, scaler, flags, _lib.stream_ptr())
+        else:
+            rc = _lib.lib().sod_sgd_momentum(f.param.data_ptr(), f.mom.data_ptr(), f.grad.data_ptr(), g16, s16, f.numel,
+                                             segs, n, lr_dev, float(self.inv_scale), finf, flags, _lib.stream_ptr())
         _lib.check(rc, "sod_sgd_momentum")
 
-    def _launch_allreduce(self, segs, n, lr_dev, g16, s16, finf):
+    def _launch_allreduce(self, segs, n, lr_dev, g16, s16, finf, scaler=None):
         f = self.flat
-        rc = _lib.lib().sod_allreduce_sgd(f.arena.ref, f.grad_off, f.grad16_off if g16 is not None else 0, f.param_off,
-                                          f.mom.data_ptr(), s16, f.numel, segs, n, lr_dev, float(self.inv_scale), finf,
-                                          _lib.SOD_SGD_ZERO_GRAD, _lib.stream_ptr())
+        flags = _lib.SOD_SGD_ZERO_GRAD | f.flags16
+        g16_off = f.grad16_off if g16 is not None else 0
+        if scaler is not None:
+            rc = _lib.lib().sod_allreduce_sgd_scaler(f.arena.ref, f.grad_off, g16_off, f.param_off, f.mom.data_ptr(), s16,
+                                                     f.numel, segs, n, lr_dev, scaler, flags, _lib.stream_ptr())
+        else:
+            rc = _lib.lib().sod_allreduce_sgd(f.arena.ref, f.grad_off, g16_off, f.param_off, f.mom.data_ptr(), s16, f.numel,
+                                              segs, n, lr_dev, float(self.inv_scale), finf, flags, _lib.stream_ptr())
         _lib.check(rc, "sod_allreduce_sgd")
 
     def gather_momentum(self) -> None:
@@ -490,19 +590,32 @@ class FusedAdam(FusedOptimizer):
         return _lib.sod_adam_segment(b, e, float(g["lr"]), float(g["weight_decay"]), float(b1), float(b2), float(g["eps"]),
                                      flags)
 
-    def _launch_local(self, segs, n, lr_dev, g16, s16, finf):
+    def _launch_local(self, segs, n, lr_dev, g16, s16, finf, scaler=None):
         f = self.flat
-        rc = _lib.lib().sod_adam(f.param.data_ptr(), f.mom.data_ptr(), self.exp_avg_sq.data_ptr(), f.grad.data_ptr(), g16,
-                                 s16, f.numel, segs, n, lr_dev, self.step_dev.data_ptr(), float(self.inv_scale), finf,
-                                 _lib.SOD_SGD_ZERO_GRAD, _lib.stream_ptr())
+        flags = _lib.SOD_SGD_ZERO_GRAD | f.flags16
+        if scaler is not None:
+            rc = _lib.lib().sod_adam_scaler(f.param.data_ptr(), f.mom.data_ptr(), self.exp_avg_sq.data_ptr(), f.grad.data_ptr(),
+                                            g16, s16, f.numel, segs, n, lr_dev, self.step_dev.data_ptr(), scaler, flags,
+                                            _lib.stream_ptr())
+        else:
+            rc = _lib.lib().sod_adam(f.param.data_ptr(), f.mom.data_ptr(), self.exp_avg_sq.data_ptr(), f.grad.data_ptr(), g16,
+                                     s16, f.numel, segs, n, lr_dev, self.step_dev.data_ptr(), float(self.inv_scale), finf,
+                                     flags, _lib.stream_ptr())
         _lib.check(rc, "sod_adam")
 
-    def _launch_allreduce(self, segs, n, lr_dev, g16, s16, finf):
+    def _launch_allreduce(self, segs, n, lr_dev, g16, s16, finf, scaler=None):
         f = self.flat
-        rc = _lib.lib().sod_allreduce_adam(f.arena.ref, f.grad_off, f.grad16_off if g16 is not None else 0, f.param_off,
-                                           f.mom.data_ptr(), self.exp_avg_sq.data_ptr(), s16, f.numel, segs, n, lr_dev,
-                                           self.step_dev.data_ptr(), float(self.inv_scale), finf, _lib.SOD_SGD_ZERO_GRAD,
-                                           _lib.stream_ptr())
+        flags = _lib.SOD_SGD_ZERO_GRAD | f.flags16
+        g16_off = f.grad16_off if g16 is not None else 0
+        if scaler is not None:
+            rc = _lib.lib().sod_allreduce_adam_scaler(f.arena.ref, f.grad_off, g16_off, f.param_off, f.mom.data_ptr(),
+                                                      self.exp_avg_sq.data_ptr(), s16, f.numel, segs, n, lr_dev,
+                                                      self.step_dev.data_ptr(), scaler, flags, _lib.stream_ptr())
+        else:
+            rc = _lib.lib().sod_allreduce_adam(f.arena.ref, f.grad_off, g16_off, f.param_off, f.mom.data_ptr(),
+                                               self.exp_avg_sq.data_ptr(), s16, f.numel, segs, n, lr_dev,
+                                               self.step_dev.data_ptr(), float(self.inv_scale), finf, flags,
+                                               _lib.stream_ptr())
         _lib.check(rc, "sod_allreduce_adam")
 
     def group_steps(self) -> list[int]:

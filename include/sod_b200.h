@@ -62,6 +62,13 @@ int sod_loss_bce_cel_fwd_bwd(const void* logits, int logits_dtype, const void* m
                              void* grad_logits, int grad_dtype, float* scalars_out, int64_t n,
                              int reduction_sum, float w_bce, float w_cel, float grad_scale, float eps,
                              int mode, void* workspace, size_t workspace_bytes, void* stream);
+/* the same with grad = (*grad_scale_dev) * grad_scale * d total / d logits, rounded once to the logits dtype: the amp loss
+ * scale is applied before the rounding (fp16 logits at a mean over millions of pixels would otherwise round the unscaled
+ * gradient, ≈1/n, into fp16's subnormal range).  grad_scale_dev: device fp32 scalar, read at execution time. */
+int sod_loss_bce_cel_fwd_bwd_scaled(const void* logits, int logits_dtype, const void* mask, int mask_dtype,
+                                    void* grad_logits, int grad_dtype, float* scalars_out, int64_t n,
+                                    int reduction_sum, float w_bce, float w_cel, float grad_scale, const float* grad_scale_dev,
+                                    float eps, int mode, void* workspace, size_t workspace_bytes, void* stream);
 /* grad *= *scale_dev (device scalar): only for the case where the loss is not the root of backward */
 int sod_scale_by_device_scalar(void* grad, int dtype, int64_t n, const float* scale_dev, void* stream);
 
@@ -130,7 +137,9 @@ enum { SOD_SGD_ZERO_GRAD = 1, SOD_ALGO_NO_MULTIMEM = 2,
        SOD_BN_L2_HINTS = 64 /* syncbn_bwd: L2 eviction-priority hints on the bulk copies — evict-last for chunks that
                                are fetched twice, evict-first for last uses */,
        SOD_BN_LAUNCH_COOP = 128 /* syncbn_fwd/bwd: cooperative launch (driver-guaranteed co-residency of the grid) */,
-       SOD_BN_LAUNCH_PDL = 256 /* syncbn_fwd/bwd: programmatic dependent launch (prologue overlaps the producer's tail) */ };
+       SOD_BN_LAUNCH_PDL = 256 /* syncbn_fwd/bwd: programmatic dependent launch (prologue overlaps the producer's tail) */,
+       SOD_GRAD16_F16 = 512 /* step kernels, sod_grad_merge_bf16, sod_grad_check_ranges: `grad16` and `shadow16` hold fp16
+                               (amp with dtype fp16) instead of bf16; the shadow is rounded to nearest, = param.half() */ };
 
 /* lr_dev (device, fp32[nseg], may be NULL): when given, the learning rate of segment i is read from lr_dev[i] at
  * execution time instead of segs[i].lr — a captured CUDA graph then follows CustomScheduler
@@ -176,6 +185,41 @@ int sod_allreduce_adam(const sod_comm* comm, uint64_t grad_off, uint64_t grad16_
                        int nseg, const float* lr_dev, int32_t* step_dev, float inv_scale,
                        const uint32_t* found_inf, int flags, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * (1c) device-resident dynamic loss scale — apex amp O1 with fp16 (train.py:183,299): initial scale 2^16; a step whose
+ *      gradients hold an inf or NaN is skipped and halves the scale (never below 1); `growth_interval` clean steps in a row
+ *      double it.  The step entry points below are the four above with `sod_loss_scaler* scaler` in place of
+ *      (inv_scale, found_inf): they read found_inf and 1/scale at execution time, and the last CTA applies the rules
+ *      (ticket, like step_dev of sod_adam):
+ *        overflow: scale = max(scale/2, 1), unskipped = 0      clean: unskipped += 1, scale *= 2 when unskipped % growth_interval == 0
+ *      found_inf is left set to the step's verdict; the caller clears it before the next step's first check (with
+ *      world > 1: after the previous step, which stream order gives).  A captured CUDA graph replays the whole protocol with
+ *      no host round trip.  One scaler per stream at a time; `ticket` starts at 0 and is left at 0.
+ * world > 1: `scaler` lives in the arena (the same offset on every rank); after its start barrier the kernel ORs the
+ * found_inf words of all ranks, so every rank skips or steps on the same verdict and the scalers stay bit-identical.
+ * ------------------------------------------------------------------------------------------------ */
+typedef struct {
+    uint32_t found_inf;        /* non-zero: a gradient of this step is inf/NaN (OR-ed in by the checks below) */
+    float scale;
+    int32_t unskipped;         /* clean steps since the last overflow (apex's `unskipped`) */
+    int32_t growth_interval;
+    uint32_t ticket;
+    uint32_t reserved[3];
+} sod_loss_scaler;
+int sod_sgd_momentum_scaler(float* param, float* mom, float* grad, void* grad16, void* shadow16, int64_t n,
+                            const sod_sgd_segment* segs, int nseg, const float* lr_dev, sod_loss_scaler* scaler, int flags,
+                            void* stream);
+int sod_allreduce_sgd_scaler(const sod_comm* comm, uint64_t grad_off, uint64_t grad16_off, uint64_t param_off, float* mom,
+                             void* shadow16, int64_t n, const sod_sgd_segment* segs, int nseg, const float* lr_dev,
+                             sod_loss_scaler* scaler, int flags, void* stream);
+int sod_adam_scaler(float* param, float* exp_avg, float* exp_avg_sq, float* grad, void* grad16, void* shadow16, int64_t n,
+                    const sod_adam_segment* segs, int nseg, const float* lr_dev, int32_t* step_dev, sod_loss_scaler* scaler,
+                    int flags, void* stream);
+int sod_allreduce_adam_scaler(const sod_comm* comm, uint64_t grad_off, uint64_t grad16_off, uint64_t param_off,
+                              float* exp_avg, float* exp_avg_sq, void* shadow16, int64_t n, const sod_adam_segment* segs,
+                              int nseg, const float* lr_dev, int32_t* step_dev, sod_loss_scaler* scaler, int flags,
+                              void* stream);
+
 /* Multi-tensor gather of bf16 gradients into the flat bf16 gradient buffer (`grad16` above): item i copies
  * numel elements from the dense tensor `src` to dst16[dst_offset ...] (dst_offset % 8 == 0).  Replaces the
  * per-parameter accumulate kernels autograd launches at the end of backward (train.py:302): the weight gradients are
@@ -186,10 +230,26 @@ typedef struct {
     int64_t dst_offset, numel;
 } sod_gather_item;
 int sod_grad_gather16(const sod_gather_item* items, int nitems, void* dst16, int64_t dst_elems, void* stream);
-/* grad[i] += float(grad16[i]); grad16[i] = 0   (world>1 pre-pass, one launch over the flat buffers) */
+/* the same gather for dtype SOD_BF16 or SOD_F16, which also does *found_inf |= any(!isfinite(what it copied)): the amp
+ * overflow check of the stolen weight gradients costs no pass of its own */
+int sod_grad_gather16_checked(const sod_gather_item* items, int nitems, void* dst16, int64_t dst_elems, int dtype,
+                              uint32_t* found_inf, void* stream);
+/* grad[i] += float(grad16[i]); grad16[i] = 0   (world>1 pre-pass, one launch over the flat buffers); sod_grad_merge16 is the
+ * same with `flags` (SOD_GRAD16_F16: grad16 is fp16) */
 int sod_grad_merge_bf16(float* grad, void* grad16, int64_t n, void* stream);
+int sod_grad_merge16(float* grad, void* grad16, int64_t n, int flags, void* stream);
 /* *found_inf |= any(!isfinite(grad)) — the amp overflow check (train.py:299), one read of grad */
 int sod_grad_nonfinite(const float* grad, int64_t n, uint32_t* found_inf, void* stream);
+/* the amp overflow check of the gradients the checked gather does not see: range i is grad16[begin, end) when its flags
+ * carry SOD_SEG_GRAD16 (fp16 with SOD_GRAD16_F16 in `flags`, else bf16), grad[begin, end) otherwise.  Ranges need no
+ * alignment; any number of them (one launch per SOD_CHECK_MAX_RANGES). */
+#define SOD_CHECK_MAX_RANGES 128
+typedef struct {
+    int64_t begin, end;
+    int32_t flags;
+} sod_check_range;
+int sod_grad_check_ranges(const float* grad, const void* grad16, int64_t n, const sod_check_range* ranges, int nranges,
+                          int flags, uint32_t* found_inf, void* stream);
 
 /* plain in-place SUM all-reduce of fp32 data at arena offset `off` (BASELINE config 5 sweep; also the
  * scalar loss mean of utils/tensor_ops.py:60-64 with scale = 1/W).  algo: 0 auto, 1 one-shot, 2 two-shot */
