@@ -9,6 +9,11 @@ Extra keys (all optional, defaults reproduce the benchmark configuration):
   channels_last   run the network in NHWC (what cuDNN's tensor-core kernels and the SyncBN kernels want)
   synthetic       train on synthetic batches of the dataloader's output contract (no dataset on this machine)
   cuda_graph      capture one iteration per (shape, lr) and replay it: one launch instead of ~700 kernel launches
+  synthetic_eval  evaluate on synthetic sets of `synthetic_eval_images` images named after the configured sets; False:
+                  read `te_data_list` / `val_data_path` from disk (a missing path is an error naming the set) and report
+                  all six metrics, with the reference's Pillow resizes reproduced bit for bit on the GPU.  Training data
+                  stays synthetic either way.  `save_pre` then writes each rank's predictions under
+                  `<output>/<exp>/pre/<set>/`.
 """
 import os
 from collections import OrderedDict
@@ -71,6 +76,7 @@ user_config = {
     "synthetic_iters_per_epoch": 20,
     "synthetic_uint8": True,      # synthetic batches as 8-bit images + GPU pre-processing kernel (pipeline.py); False: fp32 tensors from the host
     "cuda_graph": True,           # replay each iteration as one CUDA graph (one graph per input size; lr read from a device table)
+    "synthetic_eval": True,       # evaluate on synthetic sets; False: the on-disk te_data_list / val_data_path sets
     "synthetic_eval_images": 32,  # images per synthetic evaluation set (te_data_list / val_data_path names are kept as labels)
     "final_test": True,           # evaluate every test set after training, as reference train.py:273-275
 }

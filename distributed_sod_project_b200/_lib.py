@@ -26,6 +26,8 @@ SOD_BN_L2_HINTS = 64
 SOD_BN_LAUNCH_COOP = 128
 SOD_BN_LAUNCH_PDL = 256
 SOD_GRAD16_F16 = 512
+SOD_RESIZE_BILINEAR = 2
+SOD_RESIZE_BICUBIC = 3
 SOD_GATHER_MAX_ITEMS = 160
 SOD_CHECK_MAX_RANGES = 128
 SOD_ADAM_STEP_WORDS = SOD_MAX_SEGMENTS + 1
@@ -133,6 +135,12 @@ _PROTOTYPES = {
     "sod_saliency_head": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     "sod_saliency_hist": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "sod_maxpool3x3s2_bwd": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
+    "sod_saliency_head_ragged": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "sod_saliency_hist_ragged": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                           C.c_void_p, C.c_void_p]),
+    "sod_resize_u8_workspace_bytes": (C.c_size_t, [C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int]),
+    "sod_resize_u8": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
+                                C.c_int, C.c_void_p, C.c_size_t, C.c_void_p]),
 }
 
 EXPORTS = tuple(_PROTOTYPES)

@@ -93,15 +93,29 @@ __global__ void __launch_bounds__(256) preprocess_kernel(const __grid_constant__
 // ---------------------------------------------------------------------------------------------------------------
 // (b) saliency-metric statistics
 // ---------------------------------------------------------------------------------------------------------------
+// Where image b lives: a batch of equal-size images (off == nullptr: image b at b·h·w, every image h × w) or a ragged
+// batch (byte offsets and (h, w) per image).  Prediction and ground truth share the layout.
+struct MetricGeo {
+    const long long* off;
+    const int* hw;
+    int h, w;
+    __device__ __forceinline__ void get(int b, size_t& base, int& hh, int& ww) const {
+        if (off != nullptr) { base = static_cast<size_t>(off[b]); hh = hw[2 * b]; ww = hw[2 * b + 1]; }
+        else { base = static_cast<size_t>(b) * h * w; hh = h; ww = w; }
+    }
+};
+
 // pass 1, one CTA per image: min / max of the uint8 prediction, max of the uint8 ground truth (the reference divides by
 // it before thresholding, train.py:400-401), and — once that threshold is known — Σ g, Σ y·g, Σ x·g (centre of mass).
 // head[b] = {min_u, max_u, max_gt, _, n_fg, sum_y, sum_x, _} as int64
 __global__ void __launch_bounds__(512) metric_head_kernel(const unsigned char* __restrict__ pred, const unsigned char* __restrict__ gt,
-                                                          int h, int w, long long* __restrict__ head) {
+                                                          const MetricGeo geo, long long* __restrict__ head) {
     __shared__ int s_min, s_max, s_gmax;
     __shared__ unsigned long long s_n, s_y, s_x;
     const int b = blockIdx.x;
-    const size_t base = static_cast<size_t>(b) * h * w;
+    size_t base;
+    int h, w;
+    geo.get(b, base, h, w);
     if (threadIdx.x == 0) { s_min = 255; s_max = 0; s_gmax = 0; s_n = 0; s_y = 0; s_x = 0; }
     __syncthreads();
     int mn = 255, mx = 0, gm = 0;
@@ -131,13 +145,15 @@ __global__ void __launch_bounds__(512) metric_head_kernel(const unsigned char* _
 // pass 2, several CTAs per image: joint histogram hist[b][quadrant][gt_bin][k], k = u - min_u, quadrants split at
 // (cy[b], cx[b]) — the host derives them from pass 1 exactly as the reference does (int(round(centre)) + 1)
 __global__ void __launch_bounds__(256) metric_hist_kernel(const unsigned char* __restrict__ pred, const unsigned char* __restrict__ gt,
-                                                          int h, int w, const long long* __restrict__ head,
+                                                          const MetricGeo geo, const long long* __restrict__ head,
                                                           const int* __restrict__ split_yx, unsigned* __restrict__ hist) {
     __shared__ unsigned s_h[4 * 2 * 256];
     const int b = blockIdx.y;
     for (int i = threadIdx.x; i < 2048; i += blockDim.x) s_h[i] = 0;
     __syncthreads();
-    const size_t base = static_cast<size_t>(b) * h * w;
+    size_t base;
+    int h, w;
+    geo.get(b, base, h, w);
     const int mn = static_cast<int>(head[static_cast<size_t>(b) * 8 + 0]);
     const int gmax = static_cast<int>(head[static_cast<size_t>(b) * 8 + 2]);
     const int cy = split_yx[2 * b], cx = split_yx[2 * b + 1];
@@ -209,14 +225,32 @@ extern "C" int sod_saliency_quantize(const void* pred, int dtype, void* out_u8, 
     });
 }
 
+namespace sod {
+namespace {
+
+int launch_head(const void* pred_u8, const void* gt_u8, int n, MetricGeo geo, int64_t* head, void* stream) {
+    metric_head_kernel<<<n, 512, 0, static_cast<cudaStream_t>(stream)>>>(static_cast<const unsigned char*>(pred_u8),
+                                                                       static_cast<const unsigned char*>(gt_u8), geo,
+                                                                       reinterpret_cast<long long*>(head));
+    return static_cast<int>(cudaGetLastError());
+}
+
+int launch_hist(const void* pred_u8, const void* gt_u8, int n, MetricGeo geo, int per, const int64_t* head,
+                const int32_t* split_yx, uint32_t* hist, void* stream) {
+    metric_hist_kernel<<<dim3(per, n), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+        static_cast<const unsigned char*>(pred_u8), static_cast<const unsigned char*>(gt_u8), geo,
+        reinterpret_cast<const long long*>(head), split_yx, hist);
+    return static_cast<int>(cudaGetLastError());
+}
+
+}  // namespace
+}  // namespace sod
+
 extern "C" int sod_saliency_head(const void* pred_u8, const void* gt_u8, int n, int h, int w, int64_t* head, void* stream) {
     using namespace sod;
     SOD_CHECK_ARG(pred_u8 && gt_u8 && head && n > 0 && h > 0 && w > 0, SOD_EINVAL);
     SOD_CHECK_ARG(static_cast<long long>(h) * w < (1ll << 31), SOD_EUNSUPPORTED);
-    metric_head_kernel<<<n, 512, 0, static_cast<cudaStream_t>(stream)>>>(static_cast<const unsigned char*>(pred_u8),
-                                                                       static_cast<const unsigned char*>(gt_u8), h, w,
-                                                                       reinterpret_cast<long long*>(head));
-    return static_cast<int>(cudaGetLastError());
+    return launch_head(pred_u8, gt_u8, n, MetricGeo{nullptr, nullptr, h, w}, head, stream);
 }
 
 extern "C" int sod_saliency_hist(const void* pred_u8, const void* gt_u8, int n, int h, int w, const int64_t* head,
@@ -227,8 +261,25 @@ extern "C" int sod_saliency_hist(const void* pred_u8, const void* gt_u8, int n, 
     int per = (h * w + 256 * 16 - 1) / (256 * 16);
     if (per < 1) per = 1;
     if (per > 64) per = 64;
-    metric_hist_kernel<<<dim3(per, n), 256, 0, static_cast<cudaStream_t>(stream)>>>(
-        static_cast<const unsigned char*>(pred_u8), static_cast<const unsigned char*>(gt_u8), h, w,
-        reinterpret_cast<const long long*>(head), split_yx, hist);
-    return static_cast<int>(cudaGetLastError());
+    return launch_hist(pred_u8, gt_u8, n, MetricGeo{nullptr, nullptr, h, w}, per, head, split_yx, hist, stream);
+}
+
+extern "C" int sod_saliency_head_ragged(const void* pred_u8, const void* gt_u8, int n, const int64_t* offsets,
+                                        const int32_t* hw, int64_t* head, void* stream) {
+    using namespace sod;
+    SOD_CHECK_ARG(pred_u8 && gt_u8 && offsets && hw && head && n > 0, SOD_EINVAL);
+    return launch_head(pred_u8, gt_u8, n, MetricGeo{reinterpret_cast<const long long*>(offsets), hw, 0, 0}, head, stream);
+}
+
+extern "C" int sod_saliency_hist_ragged(const void* pred_u8, const void* gt_u8, int n, const int64_t* offsets,
+                                        const int32_t* hw, const int64_t* head, const int32_t* split_yx, uint32_t* hist,
+                                        void* stream) {
+    using namespace sod;
+    SOD_CHECK_ARG(pred_u8 && gt_u8 && offsets && hw && head && split_yx && hist && n > 0, SOD_EINVAL);
+    // image sizes live on the device: a fixed number of CTAs per image, about 4 waves in all
+    int per = (4 * dev_info().sm_count + n - 1) / n;
+    if (per < 1) per = 1;
+    if (per > 64) per = 64;
+    return launch_hist(pred_u8, gt_u8, n, MetricGeo{reinterpret_cast<const long long*>(offsets), hw, 0, 0}, per, head,
+                       split_yx, hist, stream);
 }

@@ -117,7 +117,7 @@ class SaliencyMetrics:
 
     def __init__(self, num: int | None = None, beta_for_wfm: int = 1, wfm: str | None = None, group=None):
         self.num, self.beta, self.wfm_mode, self.group = num, beta_for_wfm, wfm, group
-        self._pending: list = []          # (head int64[N,8] device, hist uint32[N,4,2,256] device, h, w)
+        self._pending: list = []          # (head int64[N,8] device, hist uint32[N,4,2,256] device, h, w, raw maps or None)
         self._sums = {k: 0.0 for k in ("mae", "meanf", "sm", "em", "wfm")}
         self._precision, self._recall = np.zeros(255), np.zeros(255)
         self._count = 0
@@ -151,14 +151,41 @@ class SaliencyMetrics:
         hist = torch.zeros((n, 4, 2, 256), dtype=torch.int32, device=p.device)
         lib, s = _lib.lib(), _lib.stream_ptr()
         _lib.check(lib.sod_saliency_head(p.data_ptr(), g.data_ptr(), n, h, w, head.data_ptr(), s), "sod_saliency_head")
-        # quadrant split = int(round(centre of mass)) + 1 (utils/saliency_metric.py:122-124); round-half-even like Python's
-        nfg = head[:, 4].clamp_min(1).double()
-        split = torch.stack([torch.round(head[:, 5].double() / nfg), torch.round(head[:, 6].double() / nfg)], dim=1).to(torch.int32) + 1
-        split = split.contiguous()
+        split = self._split(head)
         _lib.check(lib.sod_saliency_hist(p.data_ptr(), g.data_ptr(), n, h, w, head.data_ptr(), split.data_ptr(), hist.data_ptr(), s),
                    "sod_saliency_hist")
         _lib.count_launch(2)
         self._pending.append((head, hist, h, w, (p, g) if self.wfm_mode == "host" else None))
+
+    def update_ragged(self, pred, gt) -> None:
+        """pred, gt: `pipeline.Ragged` uint8 "L" batches with the same per-image sizes (the prediction already resized to
+        its ground truth's size, `pipeline.resize_u8`).  Same statistics as `update_batch`, images of any sizes in one
+        pair of launches.  Asynchronous."""
+        if not (pred.data.is_cuda and gt.data.is_cuda):
+            raise _lib.SodError("SaliencyMetrics works on CUDA tensors (no CPU fallback)")
+        if pred.channels != 1 or gt.channels != 1 or not torch.equal(pred.hw, gt.hw):
+            raise ValueError("update_ragged expects two single-channel ragged batches of the same sizes")
+        if bool((pred.hw[:, 0].long() * pred.hw[:, 1].long() >= 2 ** 31).any()):
+            raise _lib.SodError("update_ragged: images of 2^31 pixels or more are not supported")
+        n = len(pred)
+        head = torch.empty((n, 8), dtype=torch.int64, device=pred.data.device)
+        hist = torch.zeros((n, 4, 2, 256), dtype=torch.int32, device=pred.data.device)
+        lib, s = _lib.lib(), _lib.stream_ptr()
+        p, g, off, hw = pred.data.data_ptr(), gt.data.data_ptr(), pred.off_d.data_ptr(), pred.hw_d.data_ptr()
+        _lib.check(lib.sod_saliency_head_ragged(p, g, n, off, hw, head.data_ptr(), s), "sod_saliency_head_ragged")
+        split = self._split(head)
+        _lib.check(lib.sod_saliency_hist_ragged(p, g, n, off, hw, head.data_ptr(), split.data_ptr(), hist.data_ptr(), s),
+                   "sod_saliency_hist_ragged")
+        _lib.count_launch(2)
+        raw = ([pred.image(i) for i in range(n)], [gt.image(i) for i in range(n)]) if self.wfm_mode == "host" else None
+        self._pending.append((head, hist, pred.hw[:, 0].tolist(), pred.hw[:, 1].tolist(), raw))
+
+    @staticmethod
+    def _split(head: torch.Tensor) -> torch.Tensor:
+        # quadrant split = int(round(centre of mass)) + 1 (utils/saliency_metric.py:122-124); round-half-even like Python's
+        nfg = head[:, 4].clamp_min(1).double()
+        split = torch.stack([torch.round(head[:, 5].double() / nfg), torch.round(head[:, 6].double() / nfg)], dim=1).to(torch.int32) + 1
+        return split.contiguous()
 
     def update(self, pred: torch.Tensor, gt: torch.Tensor) -> None:
         """single image, reference signature (utils/saliency_metric.py:314): uint8 maps as above"""
@@ -169,7 +196,8 @@ class SaliencyMetrics:
         for head, hist, h, w, raw in self._pending:
             head_h, hist_h = head.cpu().numpy(), hist.cpu().numpy().astype(np.int64)
             for i in range(head_h.shape[0]):
-                m = metrics_from_hist(hist_h[i], head_h[i], h, w)
+                # h, w: one size for the whole batch, or one per image (ragged batches)
+                m = metrics_from_hist(hist_h[i], head_h[i], h[i] if isinstance(h, list) else h, w[i] if isinstance(w, list) else w)
                 for k in ("mae", "meanf", "sm", "em"):
                     self._sums[k] += m[k]
                 self._precision += m["precision"]

@@ -58,6 +58,80 @@ def preprocess_batch(img_u8: torch.Tensor, mask_u8: torch.Tensor | None = None, 
     return out.permute(0, 3, 1, 2), m_out          # logical NCHW over channels-last storage
 
 
+class Ragged:
+    """A batch of uint8 images of different sizes, packed back to back with no padding: `data` (flat, CUDA), `hw`
+    (int32 [n, 2] on the host), `channels` (1: "L" [h, w]; 3: "RGB" [h, w, 3]), and the device copies of the byte
+    offsets and sizes that the kernels read."""
+
+    def __init__(self, data: torch.Tensor, hw: torch.Tensor, channels: int):
+        self.hw = hw.to(torch.int32).reshape(-1, 2).contiguous()
+        self.channels = channels
+        sizes = self.hw[:, 0].long() * self.hw[:, 1].long() * channels
+        self.off = torch.cumsum(sizes, 0) - sizes                    # int64 [n], host
+        if data.numel() != int(sizes.sum()):
+            raise ValueError(f"ragged batch: {data.numel()} bytes for images of {int(sizes.sum())}")
+        self.data = data.reshape(-1)
+        dev = data.device
+        self.off_d = self.off.to(dev, non_blocking=True)
+        self.hw_d = self.hw.to(dev, non_blocking=True)
+
+    @classmethod
+    def empty(cls, hw: torch.Tensor, channels: int, device) -> "Ragged":
+        hw = hw.to(torch.int32).reshape(-1, 2)
+        n_bytes = int((hw[:, 0].long() * hw[:, 1].long()).sum()) * channels
+        return cls(torch.empty(n_bytes, dtype=torch.uint8, device=device), hw, channels)
+
+    @classmethod
+    def stack(cls, images: torch.Tensor) -> "Ragged":
+        """equal-size images uint8 [n, h, w] or [n, h, w, 3]"""
+        ch = 1 if images.dim() == 3 else images.shape[-1]
+        n, h, w = images.shape[:3]
+        return cls(images.contiguous().reshape(-1), torch.tensor([[h, w]] * n, dtype=torch.int32), ch)
+
+    def __len__(self) -> int:
+        return self.hw.shape[0]
+
+    def image(self, i: int) -> torch.Tensor:
+        h, w = int(self.hw[i, 0]), int(self.hw[i, 1])
+        o = int(self.off[i])
+        v = self.data[o:o + h * w * self.channels]
+        return v.view(h, w) if self.channels == 1 else v.view(h, w, self.channels)
+
+    def as_batch(self) -> torch.Tensor:
+        """view of an equal-size batch as [n, h, w] or [n, h, w, 3]"""
+        h, w = int(self.hw[0, 0]), int(self.hw[0, 1])
+        if not bool((self.hw == self.hw[0]).all()):
+            raise ValueError("as_batch needs images of one size")
+        return self.data.view(len(self), h, w) if self.channels == 1 else self.data.view(len(self), h, w, self.channels)
+
+
+def resize_u8(src: Ragged, hw, resample: int = _lib.SOD_RESIZE_BICUBIC) -> Ragged:
+    """Pillow's `Image.resize((w, h), resample)` (BILINEAR or BICUBIC, whole image, no reducing_gap) of every image of
+    `src` to its size in `hw` (int32 [n, 2] or one (h, w) for all), bit for bit, in one batched call
+    (csrc/resize.cu).  The reference uses it on predictions (`.resize(gt.size)`: BICUBIC, train.py:392-395) and, through
+    torchvision `Resize((S, S))`, on test images (BILINEAR, utils/dataset.py:97-104)."""
+    if not src.data.is_cuda:
+        raise _lib.SodError("resize_u8 needs CUDA tensors (no CPU fallback)")
+    hw = torch.as_tensor(hw, dtype=torch.int32)
+    if hw.dim() == 1:
+        hw = hw[None].expand(len(src), 2)
+    hw = hw.contiguous()
+    if hw.shape != (len(src), 2) or bool((hw <= 0).any()):
+        raise ValueError("resize_u8: one positive (h, w) per image")
+    out = Ragged.empty(hw, src.channels, src.data.device)
+    lib = _lib.lib()
+    ws_bytes = lib.sod_resize_u8_workspace_bytes(len(src), src.hw.data_ptr(), hw.data_ptr(), src.channels, resample)
+    if ws_bytes == 0:
+        raise _lib.SodError(f"sod_resize_u8: unsupported channels={src.channels} / resample={resample}")
+    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=src.data.device)
+    rc = lib.sod_resize_u8(src.data.data_ptr(), src.off_d.data_ptr(), src.hw_d.data_ptr(), out.data.data_ptr(),
+                           out.off_d.data_ptr(), out.hw_d.data_ptr(), len(src), src.channels, resample, ws.data_ptr(),
+                           ws_bytes, _lib.stream_ptr())
+    _lib.check(rc, "sod_resize_u8")
+    _lib.count_launch(3)
+    return out
+
+
 class DevicePrefetcher:
     """Wraps an iterable of host batches `(img_u8 [N,H,W,3], mask_u8 [N,H,W], names)` (pinned or not) and yields
     device batches `(image, mask, names)` in the training format, one batch ahead: upload + `preprocess_batch` of batch

@@ -347,6 +347,30 @@ int sod_saliency_head(const void* pred_u8, const void* gt_u8, int n, int h, int 
 int sod_saliency_hist(const void* pred_u8, const void* gt_u8, int n, int h, int w, const int64_t* head,
                       const int32_t* split_yx, uint32_t* hist, void* stream);
 
+/* The same two metric kernels over a ragged batch: image i of pred_u8 and gt_u8 starts at byte offsets[i] and is
+ * hw[2i] × hw[2i+1] (device arrays; every h·w < 2^31).  sod_saliency_head / sod_saliency_hist are the special case of
+ * equal sizes. */
+int sod_saliency_head_ragged(const void* pred_u8, const void* gt_u8, int n, const int64_t* offsets, const int32_t* hw,
+                             int64_t* head, void* stream);
+int sod_saliency_hist_ragged(const void* pred_u8, const void* gt_u8, int n, const int64_t* offsets, const int32_t* hw,
+                             const int64_t* head, const int32_t* split_yx, uint32_t* hist, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * sod_resize_u8 — Pillow's `Image.resize((w, h), filter)` for 8-bit images, box = the whole image, reducing_gap=None,
+ * bit for bit: the reference's `ToPILImage()(out).resize(gt.size)` (BICUBIC, train.py:392-395) and torchvision
+ * `Resize((S, S))` on a PIL image (BILINEAR, utils/dataset.py:97-104).  channels 1 ("L") or 3 ("RGB", HWC).
+ * Ragged batch: image i of src starts at byte src_off[i] and is src_hw[2i] × src_hw[2i+1]; it is written at dst_off[i]
+ * as dst_hw[2i] × dst_hw[2i+1] (all four arrays on the device).  The workspace holds the per-image coefficient tables
+ * and intermediate rows; sod_resize_u8_workspace_bytes takes the same sizes as HOST arrays and returns 0 for invalid
+ * arguments.  An image whose part of the workspace does not fit in workspace_bytes is left unwritten.
+ * ------------------------------------------------------------------------------------------------ */
+#define SOD_RESIZE_BILINEAR 2     /* PIL.Image.Resampling.BILINEAR */
+#define SOD_RESIZE_BICUBIC 3      /* PIL.Image.Resampling.BICUBIC */
+size_t sod_resize_u8_workspace_bytes(int n, const int32_t* src_hw, const int32_t* dst_hw, int channels, int filter);
+int sod_resize_u8(const void* src, const int64_t* src_off, const int32_t* src_hw, void* dst, const int64_t* dst_off,
+                  const int32_t* dst_hw, int n, int channels, int filter, void* workspace, size_t workspace_bytes,
+                  void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -5,7 +5,9 @@ every set of `te_data_list`.  One process evaluates everything, or — launched 
 every rank evaluates its shard and the metrics are reduced over the ranks (the reference's author lists multi-GPU
 evaluation as an open issue, readme.md:67-69).  Metrics run on the GPU (distributed_sod_project_b200/metrics.py).
 
-Data sets are synthetic here (no dataset on this machine): `synthetic_eval_images` images per configured set name.
+Data sets are synthetic by default (`synthetic_eval_images` images per configured set name); with
+`"synthetic_eval": False` the `te_data_list` sets are read from disk (distributed_sod_project_b200/data.py) and all six of
+the reference's metrics are reported, predictions resized to each ground truth's size exactly as Pillow does.
 """
 from __future__ import annotations
 
@@ -17,6 +19,7 @@ import torch.distributed as dist
 from config import user_config
 from distributed_sod_project_b200 import network
 from distributed_sod_project_b200.checkpoint import resume_checkpoint
+from distributed_sod_project_b200.data import open_test_set
 from distributed_sod_project_b200.evaluate import shard, test_process
 from distributed_sod_project_b200.syncbn import convert_syncbn_model
 from distributed_sod_project_b200.synthetic import synth_eval_set
@@ -40,6 +43,22 @@ def main():
     model = convert_syncbn_model(model)                        # eval-mode BatchNorm through the same kernels as training
     resume_checkpoint(model=model, load_path=path_config["final_full_net"], mode="onlynet", local_rank=local)
     total_results = {}
+    if not user_config.get("synthetic_eval", True):
+        # the on-disk sets (reference test.py:51-75 with utils/dataset.py:72-122), six metrics per set
+        for data_name, data_path in user_config["rgb_data"]["te_data_list"].items():
+            loader, n_img = open_test_set(data_name, data_path, TEST_SETTING["batch_size"], user_config["num_workers"],
+                                          user_config["prefix"])
+            save_dir = os.path.join(path_config["save"], data_name) if user_config.get("save_pre", True) else None
+            results = test_process(model, loader, length=n_img, wfm="host", input_size=user_config["input_size"],
+                                   save_dir=save_dir)
+            msg = f"Results on the testset({data_name}:'{data_path}', {n_img} images over {world} rank(s)):\n{results}"
+            if local == 0:
+                write_data_to_file(msg, path_config["te_log"])
+                construct_print(msg)
+            total_results[data_name.upper()] = results
+        if world > 1:
+            dist.destroy_process_group()
+        return total_results
     for data_name in user_config["rgb_data"]["te_data_list"]:  # reference test.py:51-75
         n_img = user_config.get("synthetic_eval_images", 32)
         batches = synth_eval_set(data_name, list(shard(n_img)), TEST_SETTING["batch_size"], user_config["input_size"])

@@ -8,8 +8,10 @@ train.py:84-101) and the same construction order in `main_worker` (train.py:104-
 engine (`distributed_sod_project_b200/engine.py`).  NCCL is still initialised — it bootstraps the symmetric-memory
 rendezvous — but no NCCL collective runs inside an iteration.
 
-Out of scope here (SURVEY §2): TensorBoard / xlsx recorders, dataset decoding.  Evaluation (`test`, `_test_process`) runs
-distributed with GPU metrics (distributed_sod_project_b200/evaluate.py, metrics.py) on synthetic test sets.  When `user_config["synthetic"]` is set (or the dataset root is absent) batches come from
+Out of scope here (SURVEY §2): TensorBoard / xlsx recorders, decoding of training data.  Evaluation (`test`,
+`_test_process`) runs distributed with GPU metrics (distributed_sod_project_b200/evaluate.py, metrics.py): on synthetic
+test sets by default, on the configured on-disk sets (`te_data_list`, `val_data_path`) with `"synthetic_eval": False`
+(distributed_sod_project_b200/data.py).  When `user_config["synthetic"]` is set (or the dataset root is absent) training batches come from
 `synthetic.synth_batch`, which honours the dataloader's output contract, incl. the multi-scale `size_list` collate.
 """
 from __future__ import annotations
@@ -25,6 +27,7 @@ import torch.distributed as dist
 from config import user_config
 from distributed_sod_project_b200 import amp
 from distributed_sod_project_b200.checkpoint import resume_checkpoint, save_checkpoint
+from distributed_sod_project_b200.data import open_test_set
 from distributed_sod_project_b200.engine import Trainer
 from distributed_sod_project_b200.evaluate import shard, test_process
 from distributed_sod_project_b200.synthetic import synth_batch, synth_eval_set
@@ -142,6 +145,19 @@ def main_worker(local_rank, ngpus_per_node, world_size, args, exp_name, path_con
         here every rank evaluates its shard and the metrics are reduced over the ranks (evaluate.py)"""
         names = cfg["rgb_data"]["val_data_path"] if mode == "val" else cfg["rgb_data"]["te_data_list"]
         total_results = {}
+        if not cfg.get("synthetic_eval", True):
+            # the reference's on-disk sets (train.py:346-376), every rank its shard, six metrics as the reference reports
+            for data_name, data_path in names.items():
+                loader, n_img = open_test_set(data_name, data_path, batch_size_single_gpu, cfg["num_workers"], cfg["prefix"])
+                save_dir = os.path.join(path_config["save"], data_name) if cfg.get("save_pre", True) else None
+                results = test_process(trainer.model, loader, length=n_img, wfm="host", input_size=cfg["input_size"],
+                                       save_dir=save_dir)
+                msg = f"Results on the {mode}set({data_name}:'{data_path}', {n_img} images over {max(world_size, 1)} rank(s)):\n{results}"
+                if local_rank == 0:
+                    write_data_to_file(msg, path_config["te_log"])
+                    construct_print(msg)
+                total_results[data_name.upper()] = results
+            return total_results
         for data_name in names:
             n_img = cfg.get("synthetic_eval_images", 32)
             mine = list(shard(n_img))
