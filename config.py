@@ -7,12 +7,13 @@ exits — a fresh checkout has none).  Every other default is the reference's.
 Extra keys (all optional, defaults reproduce the benchmark configuration):
   dtype           "bf16" | "fp16" | "fp32": autocast dtype used when `use_amp` is True
   channels_last   run the network in NHWC (what cuDNN's tensor-core kernels and the SyncBN kernels want)
-  synthetic       train on synthetic batches of the dataloader's output contract (no dataset on this machine)
+  synthetic       train on synthetic batches of the dataloader's output contract; False: train on
+                  `rgb_data.tr_data_path` with the reference's resize and augmentation run on the GPU (train.py)
   cuda_graph      capture one iteration per (shape, lr) and replay it: one launch instead of ~700 kernel launches
   synthetic_eval  evaluate on synthetic sets of `synthetic_eval_images` images named after the configured sets; False:
                   read `te_data_list` / `val_data_path` from disk (a missing path is an error naming the set) and report
-                  all six metrics, with the reference's Pillow resizes reproduced bit for bit on the GPU.  Training data
-                  stays synthetic either way.  `save_pre` then writes each rank's predictions under
+                  all six metrics, with the reference's Pillow resizes reproduced bit for bit on the GPU.
+                  `save_pre` then writes each rank's predictions under
                   `<output>/<exp>/pre/<set>/`.
 """
 import os

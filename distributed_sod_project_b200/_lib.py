@@ -70,6 +70,11 @@ class sod_check_range(C.Structure):
     _fields_ = [("begin", C.c_int64), ("end", C.c_int64), ("flags", C.c_int32)]
 
 
+class sod_augment_param(C.Structure):
+    _fields_ = [("rot", C.c_double * 6), ("flip", C.c_int32), ("identity", C.c_int32), ("ops", C.c_int32 * 3),
+                ("factor", C.c_float * 3)]
+
+
 _PROTOTYPES = {
     "sod_version": (C.c_int, []),
     "sod_strerror": (C.c_char_p, [C.c_int]),
@@ -141,6 +146,9 @@ _PROTOTYPES = {
     "sod_resize_u8_workspace_bytes": (C.c_size_t, [C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int]),
     "sod_resize_u8": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
                                 C.c_int, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "sod_augment_u8_workspace_bytes": (C.c_size_t, [C.c_int]),
+    "sod_augment_u8": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.POINTER(sod_augment_param),
+                                 C.c_void_p, C.c_size_t, C.c_void_p]),
 }
 
 EXPORTS = tuple(_PROTOTYPES)

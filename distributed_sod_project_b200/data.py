@@ -1,5 +1,5 @@
-"""On-disk SOD test sets: what the reference's `ImageFolder(training=False)` + `create_loader` read (utils/dataset.py:22-122,
-consumed at train.py:338-417), with everything after decoding on the GPU.
+"""On-disk SOD training and test sets: what the reference's `ImageFolder` + `create_loader` read
+(utils/dataset.py:22-156, consumed at train.py:121-138 and 338-417), with everything after decoding on the GPU.
 
 Listing follows the reference's rules:
   - `root` is a folder with `Image/` and `Mask/`, or a list file whose lines start with `<dir>/<name>`, read as
@@ -9,8 +9,9 @@ Listing follows the reference's rules:
 Pairs come sorted by mask name, so every rank sees the same order (the metrics are means: order does not change them).
 
 Workers only decode, at the original size: `Image.open(...).convert("RGB")` for images and `.convert("L")` for ground
-truths.  The collate packs both into ragged uint8 batches (`EvalBatch`); the device side (`evaluate.test_process`)
-resizes, normalises, runs the model, resizes the predictions back and histograms them.
+truths.  The collate packs both into ragged uint8 batches (`EvalBatch`, for training batches too); the device side
+(`evaluate.test_process`) resizes, normalises, runs the model, resizes the predictions back and histograms them, or
+(`pipeline.TrainPrefetcher`) resizes, augments and normalises the training batch.
 """
 from __future__ import annotations
 
@@ -113,6 +114,24 @@ def make_eval_loader(root: str, batch_size: int, indices=None, num_workers: int 
     loader = torch.utils.data.DataLoader(ds, batch_size=batch_size, shuffle=False, num_workers=num_workers, collate_fn=collate,
                                          pin_memory=torch.cuda.is_available(), drop_last=False)
     return loader, len(pairs)
+
+
+def make_train_loader(root: str, batch_size: int, world_size: int = 1, rank: int = 0, num_workers: int = 0,
+                      prefix=(".jpg", ".png"), seed: int = 0):
+    """this rank's DataLoader of ragged `EvalBatch` training batches of the reference's training set `root`
+    (utils/dataset.py:72-95, train.py:121-138): the workers only decode; resizing and augmentation run on the GPU
+    (`pipeline.TrainPrefetcher`).  Sampling is `DistributedSampler`'s: a shuffle from seed + epoch (`sampler.set_epoch`),
+    padded to a multiple of the world size, this rank's slice, and only full batches.  A missing path is an error naming
+    it: there is no fall-back to synthetic data."""
+    if not root or not os.path.exists(root):
+        raise FileNotFoundError(f"training set (tr_data_path): {root!r} does not exist")
+    ds = EvalFolder(list_pairs(root, prefix))
+    sampler = torch.utils.data.DistributedSampler(ds, num_replicas=world_size, rank=rank, shuffle=True, seed=seed)
+    loader = torch.utils.data.DataLoader(ds, batch_size=batch_size, sampler=sampler, num_workers=num_workers, collate_fn=collate,
+                                         pin_memory=torch.cuda.is_available(), drop_last=True)
+    if len(loader) == 0:
+        raise ValueError(f"training set {root!r}: {len(ds)} images give no batch of {batch_size} on each of {world_size} rank(s)")
+    return loader
 
 
 def open_test_set(data_name: str, data_path: str, batch_size: int, num_workers: int = 0, prefix=(".jpg", ".png")):

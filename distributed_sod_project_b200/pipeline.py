@@ -5,17 +5,21 @@ Reference, per sample on DataLoader workers: PIL decode → joint resize / flip 
 Normalize; then the collate function stacks fp32 tensors and — for multi-scale training — resizes the stacked batch
 with `F.interpolate` (bilinear image, nearest mask) on the CPU; the fp32 batch (16 B per pixel) is pinned and copied.
 
-Here the PIL part (decode and the geometric / colour transforms that produce 8-bit images) stays on the workers and the
-batch stays uint8 until it is on the device: `preprocess_batch` is ONE kernel (csrc/pipeline.cu) doing ToTensor,
-Normalize, the optional horizontal flip and the collate's resize, and writing the image channels-last.  4 B per pixel
-cross PCIe instead of 16.  `DevicePrefetcher` is the `BackgroundGenerator(tr_loader, max_prefetch=2)` of train.py:285
-with a copy stream: batch k+1 is uploaded and pre-processed while iteration k runs.
+Here only decoding stays on the workers and the batch stays uint8 until it is on the device: `preprocess_batch` is ONE
+kernel (csrc/pipeline.cu) doing ToTensor, Normalize, the optional horizontal flip and the collate's resize, and writing
+the image channels-last.  4 B per pixel cross PCIe instead of 16.  `DevicePrefetcher` is the
+`BackgroundGenerator(tr_loader, max_prefetch=2)` of train.py:285 with a copy stream: batch k+1 is uploaded and
+pre-processed while iteration k runs.  For on-disk training sets `TrainPrefetcher` also runs the reference's
+JointResize (`resize_u8`) and flip / rotate / ColorJitter (`augment_u8`) on the GPU, bit for bit as Pillow computes them.
 """
 from __future__ import annotations
 
 import ctypes as C
+import math
 import random
+from dataclasses import dataclass
 
+import numpy as np
 import torch
 
 from . import _lib
@@ -132,6 +136,80 @@ def resize_u8(src: Ragged, hw, resample: int = _lib.SOD_RESIZE_BICUBIC) -> Ragge
     return out
 
 
+@dataclass
+class AugmentParams:
+    """per-sample parameters of the reference's training augmentation for a batch of `size`² samples: `flip` (bool),
+    `angle` (degrees, as `RandomRotate` draws it), `order` (the three ColorJitter op ids — 0 brightness, 1 contrast,
+    2 saturation — in application order) and `factor` (float32 brightness, contrast, saturation factors)"""
+    size: int
+    flip: list
+    angle: list
+    order: list
+    factor: list
+
+    def __len__(self) -> int:
+        return len(self.flip)
+
+    def c_array(self):
+        arr = (_lib.sod_augment_param * len(self))()
+        for i, p in enumerate(arr):
+            m, ident = rotate_matrix(self.angle[i], self.size, self.size)
+            p.rot[:] = m
+            p.flip, p.identity = int(bool(self.flip[i])), int(ident)
+            p.ops[:] = [int(o) for o in self.order[i]]
+            p.factor[:] = [float(f) for f in self.factor[i]]
+        return arr
+
+
+def rotate_matrix(angle: float, w: int, h: int):
+    """Pillow's `Image.rotate(angle)` (no expand, centre, translate) output → input affine matrix, computed with
+    Pillow's own formula → (6 coefficients, identity); identity when `angle % 360 == 0`, where Pillow copies"""
+    angle = angle % 360.0
+    if angle == 0:
+        return [1.0, 0.0, 0.0, 0.0, 1.0, 0.0], True
+    cx, cy = w / 2, h / 2
+    angle = -math.radians(angle)
+    m = [round(math.cos(angle), 15), round(math.sin(angle), 15), 0.0, round(-math.sin(angle), 15), round(math.cos(angle), 15), 0.0]
+    m[2], m[5] = m[0] * -cx + m[1] * -cy + m[2], m[3] * -cx + m[4] * -cy + m[5]
+    m[2] += cx
+    m[5] += cy
+    return m, False
+
+
+def draw_augment_params(n: int, size: int, rng: torch.Generator) -> AugmentParams:
+    """the reference's random draws for n samples, from `rng`: flip with probability 0.5 (`RandomHorizontallyFlip`),
+    angle = U[0, 1)·2·10 − 10 (`RandomRotate(10)`), a uniformly random order of brightness / contrast / saturation
+    (torchvision's `randperm(4)` with hue absent) and three factors U[0.9, 1.1] in float32 (`ColorJitter(0.1, 0.1, 0.1)`)"""
+    flip = (torch.rand(n, generator=rng, dtype=torch.float64) < 0.5).tolist()
+    angle = [r * 2 * 10 - 10 for r in torch.rand(n, generator=rng, dtype=torch.float64).tolist()]
+    order = torch.rand(n, 3, generator=rng).argsort(dim=1).tolist()
+    factor = torch.empty(n, 3).uniform_(0.9, 1.1, generator=rng).tolist()
+    return AugmentParams(size, flip, angle, order, factor)
+
+
+def augment_u8(img_u8: torch.Tensor, mask_u8: torch.Tensor, params: AugmentParams):
+    """the reference's `RandomHorizontallyFlip` → `RandomRotate(10)` → `ColorJitter(0.1, 0.1, 0.1)` on equal-size
+    batches, img_u8 uint8 [n, S, S, 3] and mask_u8 uint8 [n, S, S] on the GPU, bit for bit as Pillow and torchvision
+    compute them, with the parameters of `params` (csrc/augment.cu) → new (image, mask) tensors"""
+    if not img_u8.is_cuda:
+        raise _lib.SodError("augment_u8 needs CUDA tensors (no CPU fallback)")
+    n, s = len(params), params.size
+    if img_u8.dtype != torch.uint8 or tuple(img_u8.shape) != (n, s, s, 3):
+        raise ValueError(f"img_u8 must be uint8 [{n}, {s}, {s}, 3]")
+    if mask_u8.dtype != torch.uint8 or tuple(mask_u8.shape) != (n, s, s) or mask_u8.device != img_u8.device:
+        raise ValueError(f"mask_u8 must be uint8 [{n}, {s}, {s}] on the images' device")
+    img_u8, mask_u8 = img_u8.contiguous(), mask_u8.contiguous()
+    img_out, mask_out = torch.empty_like(img_u8), torch.empty_like(mask_u8)
+    lib = _lib.lib()
+    ws_bytes = lib.sod_augment_u8_workspace_bytes(n)
+    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=img_u8.device)
+    rc = lib.sod_augment_u8(img_u8.data_ptr(), mask_u8.data_ptr(), img_out.data_ptr(), mask_out.data_ptr(), n, s,
+                            params.c_array(), ws.data_ptr(), ws_bytes, _lib.stream_ptr())
+    _lib.check(rc, "sod_augment_u8")
+    _lib.count_launch(2)
+    return img_out, mask_out
+
+
 class DevicePrefetcher:
     """Wraps an iterable of host batches `(img_u8 [N,H,W,3], mask_u8 [N,H,W], names)` (pinned or not) and yields
     device batches `(image, mask, names)` in the training format, one batch ahead: upload + `preprocess_batch` of batch
@@ -182,3 +260,43 @@ class DevicePrefetcher:
             for t in (x, m, *keep):
                 t.record_stream(torch.cuda.current_stream())
             yield x, m, names
+
+
+class TrainPrefetcher(DevicePrefetcher):
+    """`DevicePrefetcher` for on-disk training sets: wraps a DataLoader of ragged `data.EvalBatch` batches (decoded at
+    the original size) and runs the reference's whole per-sample chain on the side stream, one batch ahead: H2D,
+    `JointResize(size)` (Pillow BICUBIC for image and mask, `resize_u8`), flip / rotate / ColorJitter (`augment_u8`),
+    then `preprocess_batch` (ToTensor, Normalize, the multi-scale collate; no flip).  Yields `(image, mask, names)`.
+
+    Deviation from the reference, on purpose: the augmentation parameters are drawn in the main process from a generator
+    seeded by (seed, epoch, rank) (`set_epoch`), not by each DataLoader worker's `random` state, so a run is reproducible
+    whatever `num_workers` is.  The distributions are the reference's (`draw_augment_params`)."""
+
+    def __init__(self, loader, size: int, size_list=None, dtype: torch.dtype = torch.float32, seed: int = 0, rank: int = 0,
+                 device: torch.device | None = None):
+        super().__init__(loader, size_list=size_list, dtype=dtype, seed=seed, device=device)
+        self.size, self.seed, self.rank = size, seed, rank
+        self.set_epoch(0)
+
+    def set_epoch(self, epoch: int) -> None:
+        """the sampler's shuffle and the drawn parameters of `epoch`; the multi-scale size sequence is the same on every rank"""
+        sampler = getattr(self.loader, "sampler", None)
+        if hasattr(sampler, "set_epoch"):
+            sampler.set_epoch(epoch)
+        self.rng.seed(self.seed + epoch)
+        state = np.random.SeedSequence([self.seed, epoch, self.rank]).generate_state(2, dtype=np.uint32)
+        self.gen = torch.Generator().manual_seed(int(state[0]) << 32 | int(state[1]))
+
+    def _stage(self, batch):
+        size = self.rng.choice(self.size_list) if self.size_list else None
+        params = draw_augment_params(len(batch), self.size, self.gen)
+        with torch.cuda.stream(self.stream):
+            img = Ragged(batch.img.to(self.device, non_blocking=True), batch.img_hw, 3)
+            mask = Ragged(batch.gt.to(self.device, non_blocking=True), batch.gt_hw, 1)
+            img = resize_u8(img, (self.size, self.size), _lib.SOD_RESIZE_BICUBIC).as_batch()
+            mask = resize_u8(mask, (self.size, self.size), _lib.SOD_RESIZE_BICUBIC).as_batch()
+            img, mask = augment_u8(img, mask, params)
+            x, m = preprocess_batch(img, mask, size=size, dtype=self.dtype)
+            ready = torch.cuda.Event()
+            ready.record(self.stream)
+        return x, m, batch.names, ready, ()

@@ -371,6 +371,30 @@ int sod_resize_u8(const void* src, const int64_t* src_off, const int32_t* src_hw
                   const int32_t* dst_hw, int n, int channels, int filter, void* workspace, size_t workspace_bytes,
                   void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * sod_augment_u8 — the reference's random training augmentation after JointResize (utils/joint_transforms.py:20-48,
+ * utils/dataset.py:86-95), bit for bit, for given per-sample parameters, over n images "RGB" S×S×3 (HWC) and masks
+ * "L" S×S, each packed back to back:
+ *   RandomHorizontallyFlip → RandomRotate: img.rotate(deg, BILINEAR), mask.rotate(deg, NEAREST), fill 0 →
+ *   ColorJitter(0.1, 0.1, 0.1) on the image: brightness / contrast / saturation in ops[] order, each
+ *   Image.blend(degenerate, img, factor).
+ * `params` is a HOST array of n entries; it is validated and copied into the workspace (no host pointer is kept).
+ * rot[] is Pillow's output → input matrix of `Image.rotate(deg)` as its Python code computes it; identity = 1 when
+ * deg % 360 == 0 (Pillow copies).  ops[] is a permutation of {0: brightness, 1: contrast, 2: saturation}.
+ * Two launches over images × row tiles.  Returns SOD_EINVAL on null pointers, n <= 0, S <= 0, a workspace smaller than
+ * sod_augment_u8_workspace_bytes(n), or ops[] that is not a permutation.  src and dst must not overlap.
+ * ------------------------------------------------------------------------------------------------ */
+typedef struct sod_augment_param {
+    double rot[6];
+    int32_t flip;        /* mirror left-right before the rotation */
+    int32_t identity;
+    int32_t ops[3];
+    float factor[3];     /* brightness, contrast, saturation (indexed by op id) */
+} sod_augment_param;
+size_t sod_augment_u8_workspace_bytes(int n);
+int sod_augment_u8(const void* img, const void* mask, void* img_out, void* mask_out, int n, int size,
+                   const sod_augment_param* params, void* workspace, size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

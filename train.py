@@ -8,11 +8,16 @@ train.py:84-101) and the same construction order in `main_worker` (train.py:104-
 engine (`distributed_sod_project_b200/engine.py`).  NCCL is still initialised — it bootstraps the symmetric-memory
 rendezvous — but no NCCL collective runs inside an iteration.
 
-Out of scope here (SURVEY §2): TensorBoard / xlsx recorders, decoding of training data.  Evaluation (`test`,
-`_test_process`) runs distributed with GPU metrics (distributed_sod_project_b200/evaluate.py, metrics.py): on synthetic
-test sets by default, on the configured on-disk sets (`te_data_list`, `val_data_path`) with `"synthetic_eval": False`
-(distributed_sod_project_b200/data.py).  When `user_config["synthetic"]` is set (or the dataset root is absent) training batches come from
-`synthetic.synth_batch`, which honours the dataloader's output contract, incl. the multi-scale `size_list` collate.
+Out of scope here (SURVEY §2): TensorBoard / xlsx recorders.  Evaluation (`test`, `_test_process`) runs distributed with
+GPU metrics (distributed_sod_project_b200/evaluate.py, metrics.py): on synthetic test sets by default, on the configured
+on-disk sets (`te_data_list`, `val_data_path`) with `"synthetic_eval": False` (distributed_sod_project_b200/data.py).
+With `"synthetic": False` training reads `rgb_data.tr_data_path` (an `Image/` + `Mask/` folder or a list file, with
+`prefix`): DataLoader workers (`num_workers`) only decode, and the GPU runs the reference's JointResize(`input_size`),
+flip, RandomRotate(10), ColorJitter(0.1, 0.1, 0.1), ToTensor / Normalize and the `size_list` collate, bit for bit as
+Pillow and torchvision compute them (distributed_sod_project_b200/pipeline.py `TrainPrefetcher`).  The random
+parameters come from generators seeded by (epoch, rank) in the main process, so a run does not depend on
+`num_workers`.  A missing `tr_data_path` is an error naming it.  With `"synthetic": True` (the default) training batches
+come from `synthetic.synth_batch`, which honours the dataloader's output contract, incl. the multi-scale collate.
 """
 from __future__ import annotations
 
@@ -110,12 +115,15 @@ def main_worker(local_rank, ngpus_per_node, world_size, args, exp_name, path_con
     batch_size_single_gpu = cfg["batch_size"] // ngpus_per_node                        # reference train.py:119
 
     if not cfg.get("synthetic", True):
-        # decoding real datasets (reference utils/dataset.py:72-116, PIL + torchvision workers) is outside the hot path this
-        # repository covers: refuse loudly rather than silently train on noise
-        raise NotImplementedError('user_config["synthetic"] is False, but only the synthetic loader is wired into this train.py; '
-                                  "feed real batches through distributed_sod_project_b200.pipeline.preprocess_batch instead")
-    use_pipeline = cfg.get("synthetic_uint8", True)
-    if use_pipeline:
+        # the reference's training set (train.py:121-138): workers decode, the GPU resizes, augments and normalises one
+        # batch ahead; a missing tr_data_path is an error naming it
+        from distributed_sod_project_b200.data import make_train_loader
+        from distributed_sod_project_b200.pipeline import TrainPrefetcher
+        rank, world = (dist.get_rank(), dist.get_world_size()) if dist.is_initialized() else (0, 1)
+        source = make_train_loader(cfg["rgb_data"]["tr_data_path"], batch_size_single_gpu, world, rank, cfg["num_workers"],
+                                   cfg["prefix"])
+        loader = TrainPrefetcher(source, cfg["input_size"], size_list=cfg["size_list"], seed=0, rank=rank)
+    elif cfg.get("synthetic_uint8", True):
         # SURVEY §8f.2: uint8 batches from the (here: synthetic) workers, pinned → H2D and ToTensor / Normalize / multi-scale
         # collate as one GPU kernel, one batch ahead of the iteration (reference: BackgroundGenerator, train.py:285)
         from distributed_sod_project_b200.pipeline import DevicePrefetcher
