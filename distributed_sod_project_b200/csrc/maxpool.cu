@@ -1,8 +1,6 @@
 // maxpool.cu — MaxPool2d(kernel 3, stride 2, padding 1) of the ResNet stem (reference backbone/origin/resnet.py: `maxpool`,
 // sliced into `div_4` by backbone/origin/from_origin.py:7-15), channels-last, forward and backward.
-//
-// EXPERIMENTAL: written after round 1's GPU budget was spent — compiled and exported, but the host layer keeps it off
-// (resample.MAXPOOL_ENABLED) until it has been checked against torch on hardware.
+// On by default (resample.MAXPOOL_ENABLED; SOD_MAXPOOL=0 keeps torch's op).
 //
 // Why: on [16,64,160,160] bf16 torch's `max_pool_forward_nhwc` + `max_pool_backward_nhwc` move ≈75 MB of compulsory
 // traffic each, and the backward drags an int64 index tensor (4× the size of the bf16 output).  Here: 16-byte channel packets, one byte of window position

@@ -15,7 +15,8 @@ namespace {
 constexpr int kThreads = 256;
 
 // ×2 bilinear, align_corners=False: out[2k] = .25 in[k-1] + .75 in[k] (k=0: in[0]); out[2k+1] = .75 in[k] + .25 in[k+1]
-// (k=H-1: in[H-1]).  Returns the two source indices and the weight of the second one.
+// (k=H-1: in[H-1]).  Returns the two source indices and the weight of the second one.  At o = 0 the first tap has
+// weight 0: the forward zeroes its operand, since 0·inf would turn an infinite in[0] into NaN.
 __device__ __forceinline__ void src_of(int o, int n_in, int& i0, int& i1, float& w1) {
     const int k = o >> 1;
     if (o & 1) {
@@ -50,6 +51,14 @@ __global__ void __launch_bounds__(kThreads) upsample2x_fwd_kernel(const T* __res
         IO<T>::load8(base + (static_cast<long long>(h0) * W + w1i) * C8 * 8, b);
         IO<T>::load8(base + (static_cast<long long>(h1) * W + w0) * C8 * 8, cc);
         IO<T>::load8(base + (static_cast<long long>(h1) * W + w1i) * C8 * 8, d);
+        if (oh == 0) {                  // row tap h0 has weight 0 (see src_of)
+#pragma unroll
+            for (int k = 0; k < 8; ++k) { a[k] = 0.f; b[k] = 0.f; }
+        }
+        if (ow == 0) {                  // column tap w0 has weight 0
+#pragma unroll
+            for (int k = 0; k < 8; ++k) { a[k] = 0.f; cc[k] = 0.f; }
+        }
         const float w00 = (1.f - fh) * (1.f - fw), w01 = (1.f - fh) * fw, w10 = fh * (1.f - fw), w11 = fh * fw;
 #pragma unroll
         for (int k = 0; k < 8; ++k) o[k] = w00 * a[k] + w01 * b[k] + w10 * cc[k] + w11 * d[k];

@@ -164,7 +164,7 @@ class _Stem(nn.Sequential):
 
 
 class _StemPool(nn.MaxPool2d):
-    """the ResNet stem's MaxPool2d(3, 2, 1); routed to csrc/maxpool.cu when that (experimental) kernel is enabled"""
+    """the ResNet stem's MaxPool2d(3, 2, 1); routed to csrc/maxpool.cu when that kernel is enabled (the default)"""
 
     def forward(self, x):
         from .. import resample

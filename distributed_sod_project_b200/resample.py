@@ -131,7 +131,7 @@ class _MaxPool3x3s2(torch.autograd.Function):
 
 
 def maxpool3x3s2(x: torch.Tensor) -> torch.Tensor | None:
-    """MaxPool2d(3, stride 2, padding 1); None (caller keeps the torch op) unless the experimental kernel is enabled"""
+    """MaxPool2d(3, stride 2, padding 1); None (caller keeps the torch op) when the kernel is switched off or does not cover x"""
     if not (MAXPOOL_ENABLED and _ok(x)):
         return None
     return _MaxPool3x3s2.apply(x)

@@ -3,6 +3,8 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from oracle import resample_geometry as geo
+
 pytestmark = pytest.mark.gpu
 
 
@@ -26,23 +28,24 @@ def test_upsample2x_matches_interpolate(shape, dtype, with_add):
     from distributed_sod_project_b200 import resample
     n, c, h, w = shape
     x1 = _mk(shape, dtype, 1).requires_grad_(True)
-    x2 = x1.detach().clone().requires_grad_(True)
     lat1 = _mk((n, c, 2 * h, 2 * w), dtype, 2).requires_grad_(True) if with_add else None
     lat2 = lat1.detach().clone().requires_grad_(True) if with_add else None
     y1 = resample.upsample2x_add(x1, lat1) if with_add else resample.upsample2x(x1, (2 * h, 2 * w))
     assert y1 is not None and y1.is_contiguous(memory_format=torch.channels_last)
-    ref = F.interpolate(x2.float(), size=(2 * h, 2 * w), mode="bilinear", align_corners=False)
+    # against float64: one ulp of the dtype plus the fp32 slack of the weighted sums (test_upsample2x_past_one_grid_pass)
+    x2 = x1.detach().double().requires_grad_(True)
+    ref = F.interpolate(x2, size=(2 * h, 2 * w), mode="bilinear", align_corners=False)
+    mag = F.interpolate(x2.detach().abs(), size=(2 * h, 2 * w), mode="bilinear", align_corners=False)
     if with_add:
-        ref = ref + lat2.float()
-    tol = dict(rtol=1e-5, atol=1e-5) if dtype == torch.float32 else dict(rtol=2e-2, atol=2e-2) if dtype == torch.bfloat16 \
-        else dict(rtol=2e-3, atol=2e-3)
-    assert torch.allclose(y1.float(), ref, **tol)
+        ref = ref + lat2.double()
+        mag = mag + lat2.double().abs()
+    assert bool(((y1.double() - ref.detach()).abs() <= _ulp(ref.detach(), dtype) + 2.0 ** -20 * mag).all())
     dy = _mk((n, c, 2 * h, 2 * w), dtype, 3)
     y1.backward(dy)
-    ref.backward(dy.float())
-    btol = dict(rtol=1e-5, atol=1e-5) if dtype == torch.float32 else dict(rtol=3e-2, atol=3e-2) if dtype == torch.bfloat16 \
-        else dict(rtol=4e-3, atol=4e-3)
-    assert torch.allclose(x1.grad.float(), x2.grad.float(), **btol)
+    ref.backward(dy.double())
+    x0 = torch.zeros_like(x2).requires_grad_(True)
+    F.interpolate(x0, size=(2 * h, 2 * w), mode="bilinear", align_corners=False).backward(dy.double().abs())
+    assert bool(((x1.grad.double() - x2.grad).abs() <= _ulp(x2.grad, dtype) + 2.0 ** -20 * x0.grad).all())
     if with_add:
         assert torch.equal(lat1.grad, dy)
 
@@ -52,16 +55,14 @@ def test_upsample2x_matches_interpolate(shape, dtype, with_add):
 def test_avgpool2x2_matches_torch(shape, dtype):
     from distributed_sod_project_b200 import resample
     x1 = _mk(shape, dtype, 5).requires_grad_(True)
-    x2 = x1.detach().clone().requires_grad_(True)
+    x2 = x1.detach()
     y1 = resample.avgpool2x2(x1)
-    ref = F.avg_pool2d(x2.float(), 2, 2)
-    tol = dict(rtol=1e-6, atol=1e-6) if dtype == torch.float32 else dict(rtol=1e-2, atol=1e-2) if dtype == torch.bfloat16 \
-        else dict(rtol=1e-3, atol=1e-3)
-    assert torch.allclose(y1.float(), ref, **tol)
+    ref = F.avg_pool2d(x2.double(), 2, 2)
+    # against float64: one ulp plus the rounding of the fp32 sum of four (2⁻²² of the mean of |x|)
+    assert bool(((y1.double() - ref).abs() <= _ulp(ref, dtype) + 2.0 ** -22 * F.avg_pool2d(x2.double().abs(), 2, 2)).all())
     dy = _mk(tuple(ref.shape), dtype, 6)
     y1.backward(dy)
-    ref.backward(dy.float())
-    assert torch.allclose(x1.grad.float(), x2.grad.float(), **tol)
+    assert torch.equal(x1.grad, F.interpolate(dy.double() / 4, scale_factor=2, mode="nearest").to(dtype))   # dy/4: exact
 
 
 def test_unsupported_shapes_fall_back_and_backward_is_deterministic():
@@ -119,9 +120,10 @@ def test_colsum_matches_torch_and_is_deterministic(shape, dtype):
     g = torch.Generator().manual_seed(sum(shape))
     x = torch.randn(shape, generator=g).to(dtype).cuda().contiguous(memory_format=torch.channels_last)
     got = resample.colsum(x)
-    want = x.double().sum(dim=(0, 2, 3))
-    tol = {torch.float32: 1e-5, torch.bfloat16: 2.0 ** -8, torch.float16: 2.0 ** -11}[dtype]
-    assert float((got.double() - want).abs().max()) <= tol * float(x.double().abs().sum(dim=(0, 2, 3)).max())
+    sm = torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count
+    rows = x.permute(0, 2, 3, 1).reshape(-1, shape[1]).float().cpu().numpy()
+    want = torch.from_numpy(geo.colsum_replay(rows, sm)).to(dtype)
+    assert torch.equal(got.cpu(), want), "the column sum is not the kernel's fp32 summation order rounded once"
     assert all(torch.equal(resample.colsum(x), got) for _ in range(3))
 
 
@@ -144,6 +146,7 @@ def test_conv_with_colsum_bias_gradient_matches_autograd():
                 y.backward(dy)
                 res.append((y.detach(), xx.grad, w.grad, b.grad))
             assert torch.equal(res[0][0], res[1][0])
+            assert torch.equal(res[1][3], resample.colsum(dy).to(dtype))        # the bias gradient IS the column sum
             for a, bb in zip(res[0][1:], res[1][1:]):
                 assert float((a.float() - bb.float()).abs().max()) <= tol * max(1.0, float(a.float().abs().max()))
     finally:
