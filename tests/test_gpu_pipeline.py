@@ -22,20 +22,21 @@ def test_preprocess_batch_matches_the_reference_transforms(hs, ws, size, with_ma
     want_x, want_m = opipe.preprocess(img, mask, size=size, flip=flip)
     x, m = preprocess_batch(img.cuda(), mask.cuda() if with_mask else None, size=size, flip=flip.cuda() if with_flip else None)
     assert x.shape == want_x.shape and x.is_contiguous(memory_format=torch.channels_last)
-    # fp32 arithmetic in torch's operation order; the bilinear weights are formed the same way, sums may re-associate
-    assert float((x.cpu() - want_x).abs().max()) <= 4e-6
+    if size is None or (hs, ws) == ((size, size) if isinstance(size, int) else tuple(size)):
+        assert torch.equal(x.cpu(), want_x)                      # no resize: torch's fp32 operations exactly
+    else:
+        # the taps and λ are torch's; the 4-term blend may round differently (tests/test_gpu_data_regimes.py bounds
+        # the kernel against float64 at 1.2e-6, torch's own fp32 blend adds as much again)
+        assert float((x.cpu() - want_x).abs().max()) <= 4e-6
     if with_mask:
         assert torch.equal(m.cpu(), want_m)                      # nearest neighbour of k/255: exact
     else:
         assert m is None
-    xb, _ = preprocess_batch(img.cuda(), mask.cuda() if with_mask else None, size=size, flip=flip.cuda() if with_flip else None,
-                             dtype=torch.bfloat16)
-    assert xb.dtype == torch.bfloat16 and float((xb.float().cpu() - want_x).abs().max()) <= 2.0 ** -7 * float(want_x.abs().max())
-    # fp16 (the apex O1 input dtype): the fp32 value above rounded once, so within one fp16 ulp of the reference plus its 4e-6
-    xh, _ = preprocess_batch(img.cuda(), mask.cuda() if with_mask else None, size=size, flip=flip.cuda() if with_flip else None,
-                             dtype=torch.float16)
-    ulp16 = torch.exp2(torch.floor(torch.log2(want_x.double().abs().clamp_min(2.0 ** -14))) - 10)
-    assert xh.dtype == torch.float16 and bool(((xh.double().cpu() - want_x.double()).abs() <= ulp16 + 4e-6).all())
+    # bf16 and fp16 (the apex O1 input dtype): the fp32 output rounded once
+    for dt in (torch.bfloat16, torch.float16):
+        x16, _ = preprocess_batch(img.cuda(), mask.cuda() if with_mask else None, size=size,
+                                  flip=flip.cuda() if with_flip else None, dtype=dt)
+        assert x16.dtype == dt and torch.equal(x16, x.to(dt))
 
 
 def test_device_prefetcher_yields_every_batch_in_order():
@@ -112,9 +113,9 @@ def test_quantize_is_topilimage():
     assert torch.equal(SaliencyMetrics.quantize(p), p.mul(255).byte())         # torchvision ToPILImage: mul(255).byte()
     logits = (torch.randn(3, 1, 50, 70, generator=g) * 4).cuda()
     got, want = SaliencyMetrics.quantize(logits, apply_sigmoid=True), logits.sigmoid().mul(255).byte()
-    d = (got.int() - want.int()).abs()
-    assert int(d.max()) <= 1 and float((d > 0).float().mean()) < 2e-3            # expf vs torch.sigmoid: last-ulp ties only
-    assert SaliencyMetrics.quantize(logits.to(torch.bfloat16), apply_sigmoid=True).shape == got.shape
+    assert torch.equal(got, want)                          # torch's CUDA sigmoid is the same 1 / (1 + expf(−x))
+    lb = logits.to(torch.bfloat16)
+    assert torch.equal(SaliencyMetrics.quantize(lb, apply_sigmoid=True), lb.float().sigmoid().mul(255).byte())
 
 
 def test_distributed_style_evaluation_single_rank():
