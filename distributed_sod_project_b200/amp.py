@@ -4,7 +4,8 @@
 Default: bf16 autocast, loss scale fixed at 1.0 — bf16 has fp32's exponent range, so the dynamic
 scaler of apex O1 has nothing to do; weights, gradients and optimizer state stay fp32 ("fp32 master") exactly
 as under O1.  `dtype=torch.float16` keeps apex's dynamic-scale behaviour (init 2^16, ÷2 and skip the step on
-overflow, never below 1, ×2 after every `growth_interval` (2000) clean steps in a row).  The scaler lives on the device
+overflow, never below 1, ×2 after every `growth_interval` (2000) clean steps in a row, never above apex's
+max_loss_scale 2^24).  The scaler lives on the device
 (`sod_loss_scaler`, include/sod_b200.h): the loss gradient is formed already scaled, the overflow checks ride on the
 gradient gather, and the fused step kernel reads the verdict and 1/scale and advances the scaler itself — so an fp16
 iteration has no host round trip and replays from a CUDA graph like a bf16 one.  Both dtypes use the 16-bit shadow weights.

@@ -263,6 +263,10 @@ __device__ __forceinline__ bool nonfinite16x2(uint32_t w) {
 
 // The dynamic loss scale's rules (apex amp O1, include/sod_b200.h sod_loss_scaler), applied once per step by the last CTA
 // to get here (a ticket, as AdamRule::epilogue does), which then re-arms the ticket.  found_inf is left at the verdict.
+// Growth stops at kMaxLossScale (apex's max_loss_scale default): unbounded doubling reaches +inf from 2^127, and an
+// infinite scale makes every later step overflow while max(inf/2, 1) keeps it infinite.  A larger scale set from the
+// host still halves on overflow, as apex applies the cap on growth only.
+constexpr float kMaxLossScale = 16777216.0f;   // 2^24
 __device__ __forceinline__ void scaler_epilogue(sod_loss_scaler* sc, bool skip) {
     __shared__ bool s_last;
     __syncthreads();
@@ -278,7 +282,8 @@ __device__ __forceinline__ void scaler_epilogue(sod_loss_scaler* sc, bool skip) 
             sc->unskipped = 0;
         } else {
             sc->unskipped += 1;
-            if (sc->growth_interval > 0 && sc->unskipped % sc->growth_interval == 0) sc->scale *= 2.0f;
+            if (sc->growth_interval > 0 && sc->unskipped % sc->growth_interval == 0)
+                sc->scale = fminf(sc->scale * 2.0f, kMaxLossScale);
         }
         sc->found_inf = skip ? 1u : 0u;
         sc->ticket = 0u;
@@ -820,16 +825,20 @@ template <uint32_t kExp>
 int gather16(const sod_gather_item* items, int nitems, void* dst16, int64_t dst_elems, uint32_t* found, void* stream) {
     SOD_CHECK_ARG(nitems >= 0 && (nitems == 0 || items) && dst16 && dst_elems > 0, SOD_EINVAL);
     SOD_CHECK_ARG(aligned16(dst16), SOD_EALIGN);
+    // every item is checked before the first launch: a refusal leaves dst16 and *found untouched
+    for (int i = 0; i < nitems; ++i) {
+        const sod_gather_item& it = items[i];
+        if (it.src == nullptr || it.numel <= 0 || it.dst_offset < 0 || it.dst_offset + it.numel > dst_elems ||
+            it.numel > 0x7fffffffll)
+            return SOD_EINVAL;
+        if (it.dst_offset & 7) return SOD_EALIGN;
+    }
     for (int base = 0; base < nitems; base += kGatherMax) {
         GatherTable t;
         t.n = (nitems - base < kGatherMax) ? nitems - base : kGatherMax;
         unsigned chunks = 0;
         for (int i = 0; i < t.n; ++i) {
             const sod_gather_item& it = items[base + i];
-            if (it.src == nullptr || it.numel <= 0 || it.dst_offset < 0 || it.dst_offset + it.numel > dst_elems ||
-                it.numel > 0x7fffffffll)
-                return SOD_EINVAL;
-            if (it.dst_offset & 7) return SOD_EALIGN;
             t.src[i] = it.src;
             t.dst_off8[i] = static_cast<unsigned>(it.dst_offset >> 3);
             t.numel[i] = static_cast<unsigned>(it.numel);
@@ -891,6 +900,13 @@ extern "C" int sod_grad_check_ranges(const float* grad, const void* grad16, int6
                                      int nranges, int flags, uint32_t* found_inf, void* stream) {
     using namespace sod;
     SOD_CHECK_ARG(found_inf && n > 0 && nranges >= 0 && (nranges == 0 || ranges), SOD_EINVAL);
+    // every range is checked before the first launch: a refusal leaves *found_inf untouched
+    for (int i = 0; i < nranges; ++i) {
+        const sod_check_range& r = ranges[i];
+        const bool in16 = (r.flags & SOD_SEG_GRAD16) != 0;
+        if (r.begin < 0 || r.end < r.begin || r.end > n || r.end - r.begin > 0x7fffffffll) return SOD_EINVAL;
+        if (in16 ? grad16 == nullptr : grad == nullptr) return SOD_EINVAL;
+    }
     for (int base = 0; base < nranges; base += kCheckMax) {
         CheckTable t;
         t.n = 0;
@@ -898,8 +914,6 @@ extern "C" int sod_grad_check_ranges(const float* grad, const void* grad16, int6
         for (int i = base; i < nranges && i < base + kCheckMax; ++i) {
             const sod_check_range& r = ranges[i];
             const bool in16 = (r.flags & SOD_SEG_GRAD16) != 0;
-            if (r.begin < 0 || r.end < r.begin || r.end > n || r.end - r.begin > 0x7fffffffll) return SOD_EINVAL;
-            if (in16 ? grad16 == nullptr : grad == nullptr) return SOD_EINVAL;
             if (r.end == r.begin) continue;
             t.begin[t.n] = r.begin;
             t.numel[t.n] = static_cast<unsigned>(r.end - r.begin);

@@ -191,7 +191,8 @@ int sod_allreduce_adam(const sod_comm* comm, uint64_t grad_off, uint64_t grad16_
  *      double it.  The step entry points below are the four above with `sod_loss_scaler* scaler` in place of
  *      (inv_scale, found_inf): they read found_inf and 1/scale at execution time, and the last CTA applies the rules
  *      (ticket, like step_dev of sod_adam):
- *        overflow: scale = max(scale/2, 1), unskipped = 0      clean: unskipped += 1, scale *= 2 when unskipped % growth_interval == 0
+ *        overflow: scale = max(scale/2, 1), unskipped = 0      clean: unskipped += 1, scale = min(2*scale, 2^24) when
+ *        unskipped % growth_interval == 0 (apex's max_loss_scale; a larger scale set by the caller only halves on overflow)
  *      found_inf is left set to the step's verdict; the caller clears it before the next step's first check (with
  *      world > 1: after the previous step, which stream order gives).  A captured CUDA graph replays the whole protocol with
  *      no host round trip.  One scaler per stream at a time; `ticket` starts at 0 and is left at 0.

@@ -11,8 +11,10 @@ Follows
 * apex `amp.scale_loss` exit: grads ×1/S, step skipped if any grad is non-finite (train.py:299).
 * `CustomScheduler` — utils/pipeline_ops.py:185-232.
 
-Arithmetic is carried in fp32 (np.float32) in the same operation order as torch's kernel so the GPU
-result can be compared tightly; `sgd_step_f64` gives the exact-arithmetic answer for tolerance sizing.
+`sgd_step` carries the arithmetic in fp32 (np.float32) with every multiply and add rounded separately, in the order of
+torch's single-tensor formula; the kernel fuses them (`fmaf`), so the two differ by a few ulps.
+`oracle/optim_replay.py` is the kernel's own operation order, bit for bit; `sgd_step_f64` gives the exact-arithmetic
+answer for tolerance sizing.
 """
 from __future__ import annotations
 

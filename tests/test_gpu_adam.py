@@ -6,6 +6,7 @@ import pytest
 import torch
 
 from oracle import adam as oadam
+from oracle import optim_replay as rp
 
 pytestmark = pytest.mark.gpu
 
@@ -60,9 +61,11 @@ def test_flat_kernel_vs_oracle(n):
     assert oadam.adam_step(pe, me, ve, eff, segs, steps, inv_scale=0.5)
     assert step_dev.tolist()[:4] == steps + [0] == [1, 7, 9, 0]         # frozen count kept; ticket re-armed
     got = p.cpu().numpy()
-    np.testing.assert_allclose(got, pe, rtol=3e-6, atol=1e-6)
-    np.testing.assert_allclose(m.cpu().numpy(), me, rtol=3e-6, atol=1e-6)
-    np.testing.assert_allclose(v.cpu().numpy(), ve, rtol=3e-6, atol=1e-9)
+    # the kernel's own operation order, FMAs included (oracle/optim_replay.py): bit for bit
+    table = [dict(begin=s[0], end=s[1], lr=s[2], wd=s[3], beta1=B1, beta2=B2, eps=EPS, flags=s[4]) for s in spec]
+    rpe, (rme, rve), _, _, _ = rp.step("adam", p0, [m0, v0], g32, g16.float().numpy(), table, inv_scale=0.5, steps=[0, 6, 9])
+    for x, w in ((got, rpe), (m.cpu().numpy(), rme), (v.cpu().numpy(), rve)):
+        np.testing.assert_array_equal(x.view(np.uint32), w.view(np.uint32))
     np.testing.assert_array_equal(got[b:], p0[b:])                      # frozen range untouched, bit for bit
     np.testing.assert_array_equal(m.cpu().numpy()[b:], m0[b:])
     np.testing.assert_array_equal(v.cpu().numpy()[b:], v0[b:])
@@ -94,6 +97,10 @@ def test_overflow_skip_keeps_state_and_step_and_clears_grads():
     pe, me, ve, st = p0.cpu().numpy().copy(), np.zeros(n, np.float32), np.zeros(n, np.float32), [0]
     assert oadam.adam_step(pe, me, ve, np.ones(n, np.float32), [oadam.Segment(0, n, 0.1, 0.0, B1, B2, EPS)], st)
     np.testing.assert_allclose(p.cpu().numpy(), pe, rtol=3e-6, atol=1e-6)
+    rpe, _, _, _, _ = rp.step("adam", p0.cpu().numpy(), [np.zeros(n, np.float32)] * 2, np.ones(n, np.float32), None,
+                              [dict(begin=0, end=n, lr=0.1, wd=0.0, beta1=B1, beta2=B2, eps=EPS, flags=0)], zero_grad=False,
+                              steps=[0])
+    np.testing.assert_array_equal(p.cpu().numpy().view(np.uint32), rpe.view(np.uint32))
     assert float((p0 - p).min()) == pytest.approx(0.1, rel=1e-5)              # t = 1: the first Adam step moves by ≈ lr
 
 

@@ -12,6 +12,7 @@ import pytest
 import torch
 
 from oracle import adam as oadam
+from oracle import optim_replay as rp
 from oracle import sgd as osgd
 
 pytestmark = pytest.mark.gpu
@@ -53,11 +54,11 @@ def scaler_state(s):
 
 
 def model_step(scale, unskipped, gi, overflow):
-    """the rules the device scaler must follow (apex O1 dynamic scaling as amp.py applied them on the host)"""
+    """the rules the device scaler must follow (apex O1 dynamic scaling, growth capped at max_loss_scale = 2^24)"""
     if overflow:
         return max(scale / 2.0, 1.0), 0
     unskipped += 1
-    return (scale * 2.0 if unskipped % gi == 0 else scale), unskipped
+    return (min(scale * 2.0, 2.0 ** 24) if unskipped % gi == 0 else scale), unskipped
 
 
 # -- segments: [GRAD16 | fp32 | frozen | fp32]; sizes not multiples of the CTA tile ------------------------------------
@@ -202,6 +203,22 @@ def test_fp16_buffers_step_matches_fp32_step_and_fp64_oracle(rule, n):
     pg = a.p.double().cpu().numpy()
     tol = 1e-5 * (np.abs(p64) + np.abs(p64 - p0)) + 1e-30
     assert bool((np.abs(pg - p64) <= tol).all())
+    # the fp32 replay of the kernel's operation order (oracle/optim_replay.py): bit for bit.  Adam's lr 5e-3 segment is
+    # left out: at t = 1 its step_size sits within a few double ulps of an fp32 tie, so it hinges on the device's pow
+    table = []
+    for s in (adam_segs(n) if r == "adam" else sgd_segs(n, nest)):
+        d = dict(begin=s.begin, end=s.end, lr=s.lr, wd=s.weight_decay, flags=s.flags)
+        d.update(dict(beta1=s.beta1, beta2=s.beta2, eps=s.eps) if r == "adam" else dict(mu=s.momentum))
+        table.append(d)
+    pe, ste, _, _, _ = rp.step(r, p0, st0, g32, g16.float().numpy(), table, inv_scale=inv, steps=[0] * len(table))
+    keep = np.ones(n, bool)
+    for d in table:
+        if r == "adam" and not rp.adam_scalars_stable(d["lr"], d["beta1"], d["beta2"], 0):
+            keep[d["begin"]:d["end"]] = False
+    assert keep.mean() > 0.7
+    assert np.array_equal(a.p.cpu().numpy()[keep].view(np.uint32), pe[keep].view(np.uint32))
+    for x, w in zip(a.st, ste):
+        assert np.array_equal(x.cpu().numpy()[keep].view(np.uint32), w[keep].view(np.uint32))
 
 
 @pytest.mark.parametrize("rule", ["sgd", "adam"])

@@ -24,7 +24,7 @@ def model_step(scale, unskipped, gi, overflow):
     if overflow:
         return max(scale / 2.0, 1.0), 0
     unskipped += 1
-    return (scale * 2.0 if unskipped % gi == 0 else scale), unskipped
+    return (min(scale * 2.0, 2.0 ** 24) if unskipped % gi == 0 else scale), unskipped
 
 
 CASES = [(w, rule, bad) for w in vwh.WORLDS for rule in ("sgd", "adam") for bad in ("last", "first")]

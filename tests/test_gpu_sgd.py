@@ -3,6 +3,7 @@ import numpy as np
 import pytest
 import torch
 
+from oracle import optim_replay as rp
 from oracle import sgd as osgd
 
 pytestmark = pytest.mark.gpu
@@ -36,11 +37,11 @@ def test_flat_kernel_vs_oracle(n):
     segs = [osgd.Segment(0, a, 0.005, 5e-4, 0.9), osgd.Segment(a, b, 0.05, 5e-4, 0.9), osgd.Segment(b, n, 0, 0, frozen=True)]
     p, v, g = (torch.tensor(t, device="cuda") for t in (p0, v0, g0))
     assert _call(p, v, g, spec, inv_scale=0.5) == 0
-    pe, ve = p0.copy(), v0.copy()
-    assert osgd.sgd_step(pe, ve, g0, segs, inv_scale=0.5)
-    # fma contraction on the GPU vs separate mul/add in numpy: a couple of ulps
-    np.testing.assert_allclose(p.cpu().numpy(), pe, rtol=3e-6, atol=1e-6)
-    np.testing.assert_allclose(v.cpu().numpy(), ve, rtol=3e-6, atol=1e-6)
+    # the kernel's own operation order, FMAs included (oracle/optim_replay.py): bit for bit
+    table = [dict(begin=s[0], end=s[1], lr=s[2], wd=s[3], mu=s[4], flags=s[5]) for s in spec]
+    pe, (ve,), _, _, _ = rp.step("sgd", p0, [v0], g0, None, table, inv_scale=0.5)
+    np.testing.assert_array_equal(p.cpu().numpy().view(np.uint32), pe.view(np.uint32))
+    np.testing.assert_array_equal(v.cpu().numpy().view(np.uint32), ve.view(np.uint32))
     np.testing.assert_array_equal(p.cpu().numpy()[b:], p0[b:])       # frozen range untouched
     assert float(g.abs().max()) == 0.0                                  # SOD_SGD_ZERO_GRAD
     p64, v64 = osgd.sgd_step_f64(p0, v0, g0, segs, inv_scale=0.5)
@@ -56,6 +57,9 @@ def test_overflow_skip_keeps_state_and_clears_grads():
     found.zero_(); g.fill_(1.0)
     assert _call(p, v, g, [(0, n, 0.1, 0.0, 0.9, 0)], found=found, flags=0) == 0
     assert float(p.max()) == pytest.approx(1.0 - 0.1 * 2.8) and float(g.min()) == 1.0
+    pe, (ve,), _, _, _ = rp.step("sgd", np.ones(n, np.float32), [np.full(n, 2.0, np.float32)], np.ones(n, np.float32), None,
+                                 [dict(begin=0, end=n, lr=0.1, wd=0.0, mu=0.9, flags=0)], zero_grad=False)
+    assert np.array_equal(p.cpu().numpy(), pe) and np.array_equal(v.cpu().numpy(), ve)
 
 
 def test_grad_nonfinite():
