@@ -103,8 +103,15 @@ class _SyncBNFn(torch.autograd.Function):
             TRACE.append((n, c, h, w, pre is not None, res is not None, bool(relu)))
         y = torch.empty_like(x)  # preserves channels-last strides
         dev = x.device
-        mean = torch.empty(c, dtype=torch.float32, device=dev)
-        invstd = torch.empty(c, dtype=torch.float32, device=dev)
+        if training:
+            mean = torch.empty(c, dtype=torch.float32, device=dev)        # the kernel saves the batch statistics
+            invstd = torch.empty(c, dtype=torch.float32, device=dev)
+        elif any(ctx.needs_input_grad):
+            # eval with grad: the backward differentiates through the running statistics as they are now
+            mean = running_mean.detach().float().clone()
+            invstd = 1.0 / torch.sqrt(running_var.detach().float() + eps)
+        else:
+            mean = invstd = None
         cbs = [t for t in (cb1, cb2) if t is not None]
         cb_dtype = _lib.dtype_code(cbs[0].dtype) if cbs else 0
         if len(cbs) == 2 and cbs[0].dtype != cbs[1].dtype:
@@ -115,13 +122,15 @@ class _SyncBNFn(torch.autograd.Function):
             y.data_ptr(), _lib.dtype_code(x.dtype), weight.data_ptr(), bias.data_ptr(),
             running_mean.data_ptr() if running_mean is not None else None,
             running_var.data_ptr() if running_var is not None else None,
-            mean.data_ptr(), invstd.data_ptr(), rows, c, float(momentum), float(eps), int(relu), int(training),
+            mean.data_ptr() if training else None, invstd.data_ptr() if training else None, rows, c, float(momentum),
+            float(eps), int(relu), int(training),
             cref, soff, seq, epoch, nbt.data_ptr() if nbt is not None else None,
             cb1.data_ptr() if cb1 is not None else None, cb2.data_ptr() if cb2 is not None else None, cb_dtype,
             ws.data_ptr(), ws.numel(), DEBUG_FLAGS | _launch_flags(), _lib.stream_ptr())
         _lib.check(rc, "sod_syncbn_fwd")
         _lib.count_launch()
         ctx.relu, ctx.has_pre, ctx.has_res = bool(relu), pre is not None, res is not None
+        ctx.training = bool(training)
         ctx.weight_ref, ctx.bias_ref = weight, bias
         ctx.cb = (cb1, cb2)
         ctx.save_for_backward(x, pre, y if relu else None, weight, mean, invstd)
@@ -148,11 +157,42 @@ class _SyncBNFn(torch.autograd.Function):
             else:
                 dcb[i] = torch.zeros_like(cb)
                 ret_cb[i] = dcb[i]
-        dz, dres, dgamma, dbeta = raw_backward(_as_rows(dy).to(x.dtype), x, pre, y, weight, mean, invstd, ctx.relu, ctx.has_res,
-                                               into=(wg, bg) if direct else None, conv_bias=(cb1, cb2), dconv_bias=dcb,
-                                               bias=ctx.bias_ref)
+        if ctx.training:
+            dz, dres, dgamma, dbeta = raw_backward(_as_rows(dy).to(x.dtype), x, pre, y, weight, mean, invstd, ctx.relu,
+                                                   ctx.has_res, into=(wg, bg) if direct else None, conv_bias=(cb1, cb2),
+                                                   dconv_bias=dcb, bias=ctx.bias_ref)
+        else:
+            dz, dres, dgamma, dbeta = _eval_backward(_as_rows(dy).to(x.dtype), x, pre, y, weight, mean, invstd, ctx.relu,
+                                                     ctx.has_res, (cb1, cb2), dcb)
+            if direct:
+                wg.add_(dgamma)
+                bg.add_(dbeta)
         gw, gb = (None, None) if direct else (dgamma.to(weight.dtype), dbeta.to(weight.dtype))
         return (dz, dz if ctx.has_pre else None, dres, gw, gb, None, None, None, None, None, None, None, ret_cb[0], ret_cb[1])
+
+
+def _eval_backward(dy, x, pre, y, weight, mean, invstd, relu: bool, want_dres: bool, conv_bias, dconv_bias):
+    """backward of the eval-mode forward y = act(γ·(x + pre + cb − running_mean)·invstd + β [+ residual]) in fp32 torch ops:
+    the statistics are constants here, so dz = dout·γ·invstd with no batch-mean terms.  Off the training path (a frozen
+    BN while fine-tuning, input-gradient saliency).  Adds Σ dz into `dconv_bias`; returns (dz, dres|None, dγ, dβ)."""
+    c = x.shape[1]
+    dout = dy.float()
+    if relu:
+        dout = dout * (y > 0)
+    z = x.float() if pre is None else x.float() + pre.float()
+    for cb in conv_bias:
+        if cb is not None:
+            z = z + cb.detach().float().view(1, c, 1, 1)
+    xhat = (z - mean.view(1, c, 1, 1)) * invstd.view(1, c, 1, 1)
+    dz32 = dout * (weight.detach().float() * invstd).view(1, c, 1, 1)
+    if any(d is not None for d in dconv_bias):
+        s = dz32.sum(dim=(0, 2, 3))
+        for d in dconv_bias:
+            if d is not None:
+                d.copy_(d.float() + s)
+    dz = dz32.to(x.dtype).contiguous(memory_format=torch.channels_last)
+    dres = dout.to(x.dtype).contiguous(memory_format=torch.channels_last) if want_dres else None
+    return dz, dres, (dout * xhat).sum(dim=(0, 2, 3)), dout.sum(dim=(0, 2, 3))
 
 
 def raw_backward(dy, x, pre, y, weight, mean, invstd, relu: bool, want_dres: bool, into=None, conv_bias=(None, None),
@@ -171,6 +211,8 @@ def raw_backward(dy, x, pre, y, weight, mean, invstd, relu: bool, want_dres: boo
         dgamma = torch.empty(c, dtype=torch.float32, device=x.device)
         dbeta = torch.empty(c, dtype=torch.float32, device=x.device)
         flags = DEBUG_FLAGS | _launch_flags()
+    if any(d is not None for d in dconv_bias):
+        _lib.grad_writes += 1          # so does a folded conv bias's bound .grad (or a temporary: a harmless extra memset)
     if MASK_FROM_X and relu and not want_dres and bias is not None:
         flags |= _lib.SOD_BN_BWD_MASK_FROM_X
     if L2_HINTS:
