@@ -15,6 +15,9 @@ Extra keys (all optional, defaults reproduce the benchmark configuration):
                   all six metrics, with the reference's Pillow resizes reproduced bit for bit on the GPU.
                   `save_pre` then writes each rank's predictions under
                   `<output>/<exp>/pre/<set>/`.
+  wfm_impl        where the on-disk evaluation computes the weighted F-measure: "gpu" (scipy's distance transform, tie
+                  rule included, and the weighting as CUDA kernels) or "host" (scipy itself on each rank's images).  Both
+                  compute the same metric and agree to 1e-10 per image; "gpu" keeps evaluation about as fast as without it.
 """
 import os
 from collections import OrderedDict
@@ -79,6 +82,7 @@ user_config = {
     "cuda_graph": True,           # replay each iteration as one CUDA graph (one graph per input size; lr read from a device table)
     "synthetic_eval": True,       # evaluate on synthetic sets; False: the on-disk te_data_list / val_data_path sets
     "synthetic_eval_images": 32,  # images per synthetic evaluation set (te_data_list / val_data_path names are kept as labels)
+    "wfm_impl": "gpu",            # on-disk evaluation's weighted F-measure: "gpu" kernels or "host" scipy; same metric, within 1e-10 per image
     "final_test": True,           # evaluate every test set after training, as reference train.py:273-275
 }
 

@@ -143,7 +143,12 @@ _PROTOTYPES = {
     "sod_saliency_head_ragged": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "sod_saliency_hist_ragged": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                            C.c_void_p, C.c_void_p]),
-    "sod_resize_u8_workspace_bytes": (C.c_size_t, [C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int]),
+    "sod_saliency_wfm_workspace_bytes": (C.c_size_t, [C.c_int, C.c_void_p]),
+    "sod_saliency_wfm": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                                   C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "sod_saliency_wfm_ragged": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                          C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "sod_resize_u8_workspace_bytes":(C.c_size_t, [C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int]),
     "sod_resize_u8": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
                                 C.c_int, C.c_void_p, C.c_size_t, C.c_void_p]),
     "sod_augment_u8_workspace_bytes": (C.c_size_t, [C.c_int]),

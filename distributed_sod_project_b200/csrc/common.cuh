@@ -28,6 +28,26 @@ struct DevInfo {
 const DevInfo& dev_info();  // api.cu
 
 // ------------------------------------------------------------------------------------------------
+// saliency metrics: the layout and the ground-truth rule shared by the histogram (pipeline.cu) and the weighted
+// F-measure (wfm.cu) kernels
+// ------------------------------------------------------------------------------------------------
+// Where image b lives: a batch of equal-size images (off == nullptr: image b at b·h·w, every image h × w) or a ragged
+// batch (byte offsets and (h, w) per image).  Prediction and ground truth share the layout.
+struct MetricGeo {
+    const long long* off;
+    const int* hw;
+    int h, w;
+    __device__ __forceinline__ void get(int b, size_t& base, int& hh, int& ww) const {
+        if (off != nullptr) { base = static_cast<size_t>(off[b]); hh = hw[2 * b]; ww = hw[2 * b + 1]; }
+        else { base = static_cast<size_t>(b) * h * w; hh = h; ww = w; }
+    }
+};
+
+// gt_bin = (gt / (max + 1e-8) > 0.5): with integer gt this is 2·gt > max (the 1e-8 cannot move an integer comparison
+// unless 2·gt == max, where gt / (max + 1e-8) < 0.5 — i.e. strictly greater is exact); max == 0 → all background
+__device__ __forceinline__ bool metric_fg(int g, int gmax) { return gmax > 0 && 2 * g > gmax; }
+
+// ------------------------------------------------------------------------------------------------
 // 8-element packets: one 16-byte transaction for 16-bit types, two for fp32
 // ------------------------------------------------------------------------------------------------
 template <typename T>

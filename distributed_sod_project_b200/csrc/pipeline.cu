@@ -93,17 +93,7 @@ __global__ void __launch_bounds__(256) preprocess_kernel(const __grid_constant__
 // ---------------------------------------------------------------------------------------------------------------
 // (b) saliency-metric statistics
 // ---------------------------------------------------------------------------------------------------------------
-// Where image b lives: a batch of equal-size images (off == nullptr: image b at b·h·w, every image h × w) or a ragged
-// batch (byte offsets and (h, w) per image).  Prediction and ground truth share the layout.
-struct MetricGeo {
-    const long long* off;
-    const int* hw;
-    int h, w;
-    __device__ __forceinline__ void get(int b, size_t& base, int& hh, int& ww) const {
-        if (off != nullptr) { base = static_cast<size_t>(off[b]); hh = hw[2 * b]; ww = hw[2 * b + 1]; }
-        else { base = static_cast<size_t>(b) * h * w; hh = h; ww = w; }
-    }
-};
+// Images live where MetricGeo (common.cuh) says; the ground truth is binarised by metric_fg (common.cuh).
 
 // pass 1, one CTA per image: min / max of the uint8 prediction, max of the uint8 ground truth (the reference divides by
 // it before thresholding, train.py:400-401), and — once that threshold is known — Σ g, Σ y·g, Σ x·g (centre of mass).
@@ -125,13 +115,11 @@ __global__ void __launch_bounds__(512) metric_head_kernel(const unsigned char* _
     }
     atomicMin(&s_min, mn); atomicMax(&s_max, mx); atomicMax(&s_gmax, gm);
     __syncthreads();
-    // gt_bin = (gt / (max + 1e-8) > 0.5): with integer gt this is 2·gt > max (the 1e-8 cannot move an integer comparison
-    // unless 2·gt == max, where gt / (max + 1e-8) < 0.5 — i.e. strictly greater is exact); max == 0 → all background
     const int gmax = s_gmax;
     unsigned long long n = 0, sy = 0, sx = 0;
     for (int i = threadIdx.x; i < h * w; i += blockDim.x) {
         const int g = gt[base + i];
-        if (gmax > 0 && 2 * g > gmax) { ++n; sy += static_cast<unsigned>(i / w); sx += static_cast<unsigned>(i % w); }
+        if (metric_fg(g, gmax)) { ++n; sy += static_cast<unsigned>(i / w); sx += static_cast<unsigned>(i % w); }
     }
     atomicAdd(&s_n, n); atomicAdd(&s_y, sy); atomicAdd(&s_x, sx);
     __syncthreads();
@@ -160,7 +148,7 @@ __global__ void __launch_bounds__(256) metric_hist_kernel(const unsigned char* _
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < h * w; i += gridDim.x * blockDim.x) {
         const int y = i / w, x = i % w;
         const int q = (y >= cy ? 2 : 0) + (x >= cx ? 1 : 0);          // LT, RT, LB, RB
-        const int g = (gmax > 0 && 2 * static_cast<int>(gt[base + i]) > gmax) ? 1 : 0;
+        const int g = metric_fg(static_cast<int>(gt[base + i]), gmax) ? 1 : 0;
         atomicAdd(&s_h[(q * 2 + g) * 256 + (static_cast<int>(pred[base + i]) - mn)], 1u);
     }
     __syncthreads();

@@ -51,7 +51,8 @@ def test_process(model, batches, length: int | None = None, wfm: str | None = No
     """`_test_process` (train.py:372-417).  `batches`: iterable of (image, gt_u8) tuples or `data.EvalBatch`, holding
     THIS rank's shard; `length`: total number of images over all ranks (checked in show(), like the reference's `num`);
     `input_size`: the network's S for `EvalBatch` inputs; `save_dir`: if set, each 8-bit prediction resized to its ground
-    truth is written there as `<name>.png` (`EvalBatch` only: tuples carry no names).
+    truth is written there as `<name>.png` (`EvalBatch` only: tuples carry no names); `wfm`: None (no weighted
+    F-measure), "gpu" (csrc/wfm.cu) or "host" (scipy), see `metrics.SaliencyMetrics`.
     Returns {"MaxF","MeanF","WFM","MAE","SM","EM"}."""
     was_training = model.training
     model.eval()

@@ -9,15 +9,22 @@ are then functions of the joint histogram of (k, gt) over the four quadrants aro
 reference's, evaluated in float64 on 2048 counters per image.  `show()` sums over the ranks with one all-reduce.
 
 The weighted F-measure (utils/saliency_metric.py:232-303) needs an exact Euclidean distance transform and is the one
-metric that is NOT a histogram functional; `wfm="host"` evaluates it with scipy on the rank's own images (same code
-path as the reference), `wfm=None` (default) leaves it out of the result.
+metric that is NOT a histogram functional.  `wfm="gpu"` runs it as three more kernels per batch (`csrc/wfm.cu`: scipy's
+feature transform with its tie rule, then the 7×7 stencil and the weighted sums, reduced in a fixed order) and forms Q
+from three float64 sums per image on the host; it agrees with the host path to 1e-10 per image.  `wfm="host"`
+evaluates it with scipy on the rank's own images (same code path as the reference), `wfm=None` (default) leaves it
+out of the result.
 """
 from __future__ import annotations
+
+import ctypes
 
 import numpy as np
 import torch
 
 from . import _lib
+
+WFM_MODES = (None, "host", "gpu")
 
 
 # ---- formulas on histograms (host, float64) -------------------------------------------------------------------------
@@ -116,8 +123,12 @@ class SaliencyMetrics:
     reduces over the ranks.  `num` is optional (the reference pre-sizes arrays with it)."""
 
     def __init__(self, num: int | None = None, beta_for_wfm: int = 1, wfm: str | None = None, group=None):
+        if wfm not in WFM_MODES:
+            raise ValueError(f"wfm must be one of {WFM_MODES}, not {wfm!r}")
         self.num, self.beta, self.wfm_mode, self.group = num, beta_for_wfm, wfm, group
-        self._pending: list = []          # (head int64[N,8] device, hist uint32[N,4,2,256] device, h, w, raw maps or None)
+        # (head int64[N,8] device, hist uint32[N,4,2,256] device, h, w, raw maps (wfm="host") or WFM sums float64[N,4]
+        # device (wfm="gpu") or None)
+        self._pending: list = []
         self._sums = {k: 0.0 for k in ("mae", "meanf", "sm", "em", "wfm")}
         self._precision, self._recall = np.zeros(255), np.zeros(255)
         self._count = 0
@@ -155,7 +166,10 @@ class SaliencyMetrics:
         _lib.check(lib.sod_saliency_hist(p.data_ptr(), g.data_ptr(), n, h, w, head.data_ptr(), split.data_ptr(), hist.data_ptr(), s),
                    "sod_saliency_hist")
         _lib.count_launch(2)
-        self._pending.append((head, hist, h, w, (p, g) if self.wfm_mode == "host" else None))
+        extra = (p, g) if self.wfm_mode == "host" else None
+        if self.wfm_mode == "gpu":
+            extra = wfm_sums(p, g, head)
+        self._pending.append((head, hist, h, w, extra))
 
     def update_ragged(self, pred, gt) -> None:
         """pred, gt: `pipeline.Ragged` uint8 "L" batches with the same per-image sizes (the prediction already resized to
@@ -177,8 +191,10 @@ class SaliencyMetrics:
         _lib.check(lib.sod_saliency_hist_ragged(p, g, n, off, hw, head.data_ptr(), split.data_ptr(), hist.data_ptr(), s),
                    "sod_saliency_hist_ragged")
         _lib.count_launch(2)
-        raw = ([pred.image(i) for i in range(n)], [gt.image(i) for i in range(n)]) if self.wfm_mode == "host" else None
-        self._pending.append((head, hist, pred.hw[:, 0].tolist(), pred.hw[:, 1].tolist(), raw))
+        extra = ([pred.image(i) for i in range(n)], [gt.image(i) for i in range(n)]) if self.wfm_mode == "host" else None
+        if self.wfm_mode == "gpu":
+            extra = wfm_sums_ragged(pred, gt, head)
+        self._pending.append((head, hist, pred.hw[:, 0].tolist(), pred.hw[:, 1].tolist(), extra))
 
     @staticmethod
     def _split(head: torch.Tensor) -> torch.Tensor:
@@ -193,8 +209,9 @@ class SaliencyMetrics:
 
     # -- host part --------------------------------------------------------------------------------------------------
     def _drain(self) -> None:
-        for head, hist, h, w, raw in self._pending:
+        for head, hist, h, w, extra in self._pending:
             head_h, hist_h = head.cpu().numpy(), hist.cpu().numpy().astype(np.int64)
+            sums = extra.cpu().numpy() if isinstance(extra, torch.Tensor) else None
             for i in range(head_h.shape[0]):
                 # h, w: one size for the whole batch, or one per image (ragged batches)
                 m = metrics_from_hist(hist_h[i], head_h[i], h[i] if isinstance(h, list) else h, w[i] if isinstance(w, list) else w)
@@ -202,8 +219,10 @@ class SaliencyMetrics:
                     self._sums[k] += m[k]
                 self._precision += m["precision"]
                 self._recall += m["recall"]
-                if raw is not None:
-                    self._sums["wfm"] += _wfm_host(raw[0][i].cpu().numpy(), raw[1][i].cpu().numpy(), self.beta)
+                if sums is not None:
+                    self._sums["wfm"] += wfm_from_sums(*sums[i, :3], self.beta)
+                elif extra is not None:
+                    self._sums["wfm"] += _wfm_host(extra[0][i].cpu().numpy(), extra[1][i].cpu().numpy(), self.beta)
                 self._count += 1
         self._pending.clear()
 
@@ -227,6 +246,85 @@ class SaliencyMetrics:
                 "MAE": float(vec[1] / num), "SM": float(vec[3] / num), "EM": float(vec[4] / num)}
 
 
+# ---- weighted F-measure ---------------------------------------------------------------------------------------------
+def wfm_gaussian() -> np.ndarray:
+    """the reference's 7×7 MATLAB-style Gaussian with σ = 5 (utils/saliency_metric.py:279-283), float64"""
+    ax = np.arange(-3, 4, dtype=np.float64)
+    k = np.exp(-(ax[None, :] ** 2 + ax[:, None] ** 2) / (2.0 * 5 * 5))
+    k[k < np.finfo(k.dtype).eps * k.max()] = 0
+    k /= k.sum()
+    return k
+
+
+_wfm_coef = None
+
+
+def _wfm_coef_ptr() -> int:
+    """host address of the 50 doubles the WFM kernels take: the Gaussian row-major, then log(0.5)/5"""
+    global _wfm_coef
+    if _wfm_coef is None:
+        _wfm_coef = (ctypes.c_double * 50)(*np.concatenate([wfm_gaussian().reshape(-1), [np.log(0.5) / 5]]).tolist())
+    return ctypes.addressof(_wfm_coef)
+
+
+def _wfm_call(entry: str, n: int, hw_host: torch.Tensor, args_before: tuple, nearest: torch.Tensor | None, device):
+    hw_host = hw_host.to(torch.int32).contiguous()
+    lib = _lib.lib()
+    hw_p = hw_host.data_ptr()
+    ws_bytes = lib.sod_saliency_wfm_workspace_bytes(n, hw_p)
+    if ws_bytes == 0:
+        raise _lib.SodError("WFM: image sizes must be positive, below 2^31 pixels and at most 2^21 wide")
+    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=device)
+    sums = torch.empty((n, 4), dtype=torch.float64, device=device)
+    near = 0 if nearest is None else nearest.data_ptr()
+    rc = getattr(lib, entry)(*args_before, _wfm_coef_ptr(), ws.data_ptr(), ws_bytes, sums.data_ptr(), near, _lib.stream_ptr())
+    _lib.check(rc, entry)
+    _lib.count_launch()
+    return sums
+
+
+def _check_nearest(nearest, px: int, device):
+    if nearest is not None and (nearest.dtype != torch.int32 or not nearest.is_contiguous() or nearest.numel() != 2 * px
+                                or nearest.device != device):
+        raise ValueError("nearest: a contiguous int32 tensor of 2 × (total pixels) on the images' device")
+
+
+def wfm_sums(pred_u8: torch.Tensor, gt_u8: torch.Tensor, head: torch.Tensor, nearest: torch.Tensor | None = None) -> torch.Tensor:
+    """the weighted F-measure's per-image sums {ΣEw[gt], ΣEw[~gt], n_fg, 0} (float64 [N, 4], on the device) of equal-size
+    uint8 maps [N, H, W] with `head` from sod_saliency_head; `nearest` (int32 [N, H, W, 2], optional) receives scipy's
+    nearest-foreground (y, x) of every pixel.  Asynchronous."""
+    if not (pred_u8.is_cuda and gt_u8.is_cuda and head.is_cuda):
+        raise _lib.SodError("wfm_sums works on CUDA tensors (no CPU fallback)")
+    n, h, w = pred_u8.shape
+    _check_nearest(nearest, n * h * w, pred_u8.device)
+    hw = torch.tensor([[h, w]] * n, dtype=torch.int32)
+    return _wfm_call("sod_saliency_wfm", n, hw, (pred_u8.data_ptr(), gt_u8.data_ptr(), n, h, w, head.data_ptr()), nearest,
+                     pred_u8.device)
+
+
+def wfm_sums_ragged(pred, gt, head: torch.Tensor, nearest: torch.Tensor | None = None) -> torch.Tensor:
+    """`wfm_sums` of two `pipeline.Ragged` "L" batches of the same sizes; `nearest`: int32 [Σ h·w, 2], images back to
+    back.  Asynchronous."""
+    if not (pred.data.is_cuda and gt.data.is_cuda and head.is_cuda):
+        raise _lib.SodError("wfm_sums_ragged works on CUDA tensors (no CPU fallback)")
+    n = len(pred)
+    _check_nearest(nearest, int((pred.hw[:, 0].long() * pred.hw[:, 1].long()).sum()), pred.data.device)
+    args = (pred.data.data_ptr(), gt.data.data_ptr(), n, pred.off_d.data_ptr(), pred.hw_d.data_ptr(), pred.hw.data_ptr(),
+            head.data_ptr())
+    return _wfm_call("sod_saliency_wfm_ragged", n, pred.hw, args, nearest, pred.data.device)
+
+
+def wfm_from_sums(s_fg: float, s_bg: float, n_fg: float, beta: int = 1, eps: float = 1e-6) -> float:
+    """Q of utils/saliency_metric.py:292-301 from one image's sums, in float64 as `_wfm_host` forms it (0 without
+    foreground)"""
+    if n_fg == 0:
+        return 0.0
+    tpw = n_fg - s_fg
+    r = 1 - s_fg / n_fg
+    p = tpw / (eps + tpw + s_bg)
+    return float((1 + beta) * r * p / (eps + r + beta * p))
+
+
 def _wfm_host(pred_u8: np.ndarray, gt_u8: np.ndarray, beta: int = 1, eps: float = 1e-6) -> float:
     """weighted F-measure of one image on the host (utils/saliency_metric.py:255-299): the distance transform keeps it off
     the histogram path; same scipy routines as the reference."""
@@ -240,10 +338,7 @@ def _wfm_host(pred_u8: np.ndarray, gt_u8: np.ndarray, beta: int = 1, eps: float 
     err = np.abs(pred - gt)
     et = err.copy()
     et[~gt] = err[idx[0][~gt], idx[1][~gt]]
-    ax = np.arange(-3, 4, dtype=np.float64)
-    k = np.exp(-(ax[None, :] ** 2 + ax[:, None] ** 2) / (2.0 * 5 * 5))
-    k[k < np.finfo(k.dtype).eps * k.max()] = 0
-    k /= k.sum()
+    k = wfm_gaussian()
     ea = convolve(et, weights=k, mode="constant", cval=0)
     min_e = np.where(gt & (ea < err), ea, err)
     ew = min_e * np.where(gt, 1.0, 2 - np.exp(np.log(0.5) / 5 * dst))

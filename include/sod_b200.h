@@ -356,6 +356,25 @@ int sod_saliency_head_ragged(const void* pred_u8, const void* gt_u8, int n, cons
 int sod_saliency_hist_ragged(const void* pred_u8, const void* gt_u8, int n, const int64_t* offsets, const int32_t* hw,
                              const int64_t* head, const int32_t* split_yx, uint32_t* hist, void* stream);
 
+/* sod_saliency_wfm — the weighted F-measure's per-image sums (utils/saliency_metric.py:232-303) on the nearest
+ * foreground pixels scipy's `distance_transform_edt(gt == 0, return_indices=True)` picks, ties included.  Three
+ * launches; `head` is sod_saliency_head's output for the same images (it gives the binarisation and the prediction's
+ * min / max).  sums[i] = {ΣEw over the foreground, ΣEw over the background, n_fg, 0} in float64, all 0 for an image
+ * without foreground; the host forms Q from them.  The sums are reduced in a fixed order: bit-identical from run to
+ * run and whatever else is in the batch.  coef_host: 50 HOST doubles, the reference's 7×7 Gaussian (σ = 5) row-major,
+ * then log(0.5)/5.  nearest_yx (may be NULL): int32 [Σ h·w][2], images back to back in batch order, (y, x) of each
+ * pixel's nearest foreground pixel, (−1, −1) in an image without foreground.  The ragged form also takes the sizes as a
+ * HOST array hw_host (the same values as hw).  workspace: sod_saliency_wfm_workspace_bytes(n, sizes) bytes, 16-byte
+ * aligned (for the fixed form, n copies of (h, w)); it returns 0 for invalid or unsupported sizes.  SOD_EWORKSPACE and
+ * every other refusal launch nothing; images of 2^31 pixels or more, or wider than 2^21, are SOD_EUNSUPPORTED. */
+size_t sod_saliency_wfm_workspace_bytes(int n, const int32_t* hw_host);
+int sod_saliency_wfm(const void* pred_u8, const void* gt_u8, int n, int h, int w, const int64_t* head,
+                     const double* coef_host, void* workspace, size_t workspace_bytes, double* sums, int32_t* nearest_yx,
+                     void* stream);
+int sod_saliency_wfm_ragged(const void* pred_u8, const void* gt_u8, int n, const int64_t* offsets, const int32_t* hw,
+                            const int32_t* hw_host, const int64_t* head, const double* coef_host, void* workspace,
+                            size_t workspace_bytes, double* sums, int32_t* nearest_yx, void* stream);
+
 /* ------------------------------------------------------------------------------------------------
  * sod_resize_u8 — Pillow's `Image.resize((w, h), filter)` for 8-bit images, box = the whole image, reducing_gap=None,
  * bit for bit: the reference's `ToPILImage()(out).resize(gt.size)` (BICUBIC, train.py:392-395) and torchvision

@@ -49,8 +49,8 @@ def main():
             loader, n_img = open_test_set(data_name, data_path, TEST_SETTING["batch_size"], user_config["num_workers"],
                                           user_config["prefix"])
             save_dir = os.path.join(path_config["save"], data_name) if user_config.get("save_pre", True) else None
-            results = test_process(model, loader, length=n_img, wfm="host", input_size=user_config["input_size"],
-                                   save_dir=save_dir)
+            results = test_process(model, loader, length=n_img, wfm=user_config.get("wfm_impl", "gpu"),
+                                   input_size=user_config["input_size"], save_dir=save_dir)
             msg = f"Results on the testset({data_name}:'{data_path}', {n_img} images over {world} rank(s)):\n{results}"
             if local == 0:
                 write_data_to_file(msg, path_config["te_log"])

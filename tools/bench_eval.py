@@ -8,10 +8,12 @@ In one run, on the current GPU (its name and power limit are part of the output)
   PNG masks with soft edges;
 * `end_to_end_img_s`: images/s of `evaluate.test_process` over that set at the reference's test batch size (24,
   reference test.py:30) — decode on `--workers` DataLoader workers, upload, Pillow-exact resize to S², network (res50,
-  fp32, as the reference's test.py), quantize, resize back, ragged metric kernels — with the weighted F-measure on the
-  host (`wfm="host"`, six metrics as the reference reports) and without it;
+  fp32, as the reference's test.py), quantize, resize back, ragged metric kernels — without the weighted F-measure
+  (`no_wfm`), with it on the GPU (`wfm_gpu`, csrc/wfm.cu) and with it on the host (`wfm_host`, scipy); the last two
+  report all six metrics as the reference does;
 * `kernels_us`: one batch's resize and metric kernels alone (CUDA events, warmed up, `--iters` repetitions): RGB
-  BILINEAR to S², "L" BICUBIC back to each ground truth's size, ragged head + hist;
+  BILINEAR to S², "L" BICUBIC back to each ground truth's size, ragged head + hist, and the weighted F-measure's three
+  launches (`wfm_ragged`, head included as it feeds them; `wfm_alone` without it);
 * `host_reference_us`: the same batch through the reference's per-image host path — `ToPILImage`-equivalent 8-bit map,
   PIL `.resize(gt.size)` and the numpy metrics of `oracle.metrics.TotalMetric` (without the weighted F-measure).
 """
@@ -78,7 +80,7 @@ def main() -> None:
     from distributed_sod_project_b200.data import make_eval_loader
     from distributed_sod_project_b200.engine import Trainer
     from distributed_sod_project_b200.evaluate import prepare_inputs, test_process
-    from distributed_sod_project_b200.metrics import SaliencyMetrics
+    from distributed_sod_project_b200.metrics import SaliencyMetrics, wfm_sums_ragged
     from distributed_sod_project_b200.pipeline import Ragged, resize_u8
     from oracle import metrics as om
 
@@ -92,12 +94,12 @@ def main() -> None:
         warm, _ = make_eval_loader(root, args.batch, indices=range(2 * args.batch), num_workers=0)
         test_process(model, warm, length=2 * args.batch, input_size=args.size)             # cuDNN picks its algorithms
         e2e = {}
-        for wfm in (None, "host"):
+        for wfm in (None, "gpu", "host"):
             torch.cuda.synchronize()
             t0 = time.perf_counter()
             test_process(model, loader, length=n, wfm=wfm, input_size=args.size)
             torch.cuda.synchronize()
-            e2e["wfm_host" if wfm else "no_wfm"] = round(n / (time.perf_counter() - t0), 1)
+            e2e[f"wfm_{wfm}" if wfm else "no_wfm"] = round(n / (time.perf_counter() - t0), 1)
         result["end_to_end_img_s"] = e2e
 
         # one batch, kernels alone
@@ -111,10 +113,20 @@ def main() -> None:
         pred_r = Ragged.stack(pred_s)
         pred = resize_u8(pred_r, gt.hw, _lib.SOD_RESIZE_BICUBIC)
         cal = SaliencyMetrics()
+        head = torch.empty((len(gt), 8), dtype=torch.int64, device=dev)
+        lib = _lib.lib()
+
+        def head_launch():
+            _lib.check(lib.sod_saliency_head_ragged(pred.data.data_ptr(), gt.data.data_ptr(), len(gt), pred.off_d.data_ptr(),
+                                                    pred.hw_d.data_ptr(), head.data_ptr(), _lib.stream_ptr()))
+
+        head_launch()
         result["kernels_us"] = {
             "resize_rgb_bilinear_to_S": round(_events_us(lambda: resize_u8(img, (args.size, args.size), _lib.SOD_RESIZE_BILINEAR), args.iters), 1),
             "resize_l_bicubic_to_gt": round(_events_us(lambda: resize_u8(pred_r, gt.hw, _lib.SOD_RESIZE_BICUBIC), args.iters), 1),
             "metric_head_hist_ragged": round(_events_us(lambda: cal.update_ragged(pred, gt), args.iters), 1),
+            "wfm_ragged": round(_events_us(lambda: (head_launch(), wfm_sums_ragged(pred, gt, head)), args.iters), 1),
+            "wfm_alone": round(_events_us(lambda: wfm_sums_ragged(pred, gt, head), args.iters), 1),
         }
         cal._pending.clear()
 

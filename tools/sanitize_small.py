@@ -17,7 +17,7 @@ if world > 1:
 from distributed_sod_project_b200 import _lib, comm  # noqa: E402
 from distributed_sod_project_b200.loss import bce_cel_fwd_bwd  # noqa: E402
 from distributed_sod_project_b200.metrics import SaliencyMetrics  # noqa: E402
-from distributed_sod_project_b200.pipeline import preprocess_batch  # noqa: E402
+from distributed_sod_project_b200.pipeline import Ragged, preprocess_batch  # noqa: E402
 from distributed_sod_project_b200.syncbn import SyncBatchNorm  # noqa: E402
 
 cl = lambda t: t.cuda().contiguous(memory_format=torch.channels_last)  # noqa: E731
@@ -44,8 +44,12 @@ assert _lib.lib().sod_grad_gather16(items, 3, flat.data_ptr(), flat.numel(), _li
 img = torch.randint(0, 256, (2, 20, 24, 3), dtype=torch.uint8, device="cuda")
 msk = torch.randint(0, 256, (2, 20, 24), dtype=torch.uint8, device="cuda")
 preprocess_batch(img, msk, size=16)
-cal = SaliencyMetrics()
+cal = SaliencyMetrics(wfm="gpu")
 cal.update_batch(torch.randint(0, 256, (2, 20, 24), dtype=torch.uint8, device="cuda"), (torch.rand(2, 20, 24, device="cuda") > 0.6).to(torch.uint8) * 255)
+pr = Ragged(torch.randint(0, 256, (20 * 24 + 7 * 40 + 1,), dtype=torch.uint8, device="cuda"),
+            torch.tensor([[20, 24], [7, 40], [1, 1]], dtype=torch.int32), 1)
+gr = Ragged((torch.rand(pr.data.numel(), device="cuda") > 0.7).to(torch.uint8) * 255, pr.hw, 1)
+cal.update_ragged(pr, gr)
 if world > 1:
     arena = comm.Arena(payload_bytes=2 * 4 * n + 4096)
     p_off, g_off = arena.alloc(4 * n), arena.alloc(4 * n)

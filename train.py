@@ -158,8 +158,8 @@ def main_worker(local_rank, ngpus_per_node, world_size, args, exp_name, path_con
             for data_name, data_path in names.items():
                 loader, n_img = open_test_set(data_name, data_path, batch_size_single_gpu, cfg["num_workers"], cfg["prefix"])
                 save_dir = os.path.join(path_config["save"], data_name) if cfg.get("save_pre", True) else None
-                results = test_process(trainer.model, loader, length=n_img, wfm="host", input_size=cfg["input_size"],
-                                       save_dir=save_dir)
+                results = test_process(trainer.model, loader, length=n_img, wfm=cfg.get("wfm_impl", "gpu"),
+                                       input_size=cfg["input_size"], save_dir=save_dir)
                 msg = f"Results on the {mode}set({data_name}:'{data_path}', {n_img} images over {max(world_size, 1)} rank(s)):\n{results}"
                 if local_rank == 0:
                     write_data_to_file(msg, path_config["te_log"])
