@@ -26,6 +26,7 @@ SOD_BN_L2_HINTS = 64
 SOD_BN_LAUNCH_COOP = 128
 SOD_BN_LAUNCH_PDL = 256
 SOD_GRAD16_F16 = 512
+SOD_GN_GROUPS = 32
 SOD_RESIZE_BILINEAR = 2
 SOD_RESIZE_BICUBIC = 3
 SOD_GATHER_MAX_ITEMS = 160
@@ -154,6 +155,15 @@ _PROTOTYPES = {
     "sod_augment_u8_workspace_bytes": (C.c_size_t, [C.c_int]),
     "sod_augment_u8": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.POINTER(sod_augment_param),
                                  C.c_void_p, C.c_size_t, C.c_void_p]),
+    "sod_groupnorm_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int64, C.c_int, C.c_int]),
+    "sod_groupnorm_splits": (C.c_int, [C.c_int, C.c_int64, C.c_int, C.c_int]),
+    "sod_groupnorm_fwd": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
+                                    C.c_int64, C.c_int, C.c_int, C.c_float, C.c_int, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "sod_groupnorm_bwd": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
+                                    C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_size_t,
+                                    C.c_int, C.c_void_p]),
+    "sod_ws_fwd": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_float, C.c_void_p]),
+    "sod_ws_bwd": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_float, C.c_int, C.c_void_p]),
 }
 
 EXPORTS = tuple(_PROTOTYPES)

@@ -22,7 +22,7 @@ import functools
 import torch
 
 from . import _lib
-from .optim import FusedOptimizer
+from .optim import FusedOptimizer, is_plain_conv
 
 import os
 
@@ -39,12 +39,13 @@ def _install_shadow_weights(model, flat) -> int:
     """Point every Conv2d whose parameters live in `flat` at the 16-bit (bf16 or fp16) shadow copy: under autocast the
     convolution then takes its weight without a per-iteration cast kernel, and autograd accumulates the 16-bit weight
     gradient straight into the flat 16-bit gradient buffer the fused step consumes.  fp32 masters stay the module Parameters
-    (state_dict / checkpoints / optimizer groups are unaffected)."""
+    (state_dict / checkpoints / optimizer groups are unaffected).  Convolution subclasses with their own forward (the
+    weight-standardised ones) are left alone, `optim.is_plain_conv`."""
     import torch.nn as nn
     managed = {id(p) for p, _ in flat.slots}
     count = 0
     for m in model.modules():
-        if not isinstance(m, nn.Conv2d) or id(m.weight) not in managed or hasattr(m, "_sod_w16"):
+        if not is_plain_conv(m) or id(m.weight) not in managed or hasattr(m, "_sod_w16"):
             continue
         w16 = flat.view16(flat.shadow16, m.weight)
         w16.requires_grad_(m.weight.requires_grad)

@@ -1,7 +1,7 @@
 """One training iteration of the reference (train.py:284-310), wired onto the sm_90a kernels.
 
 `Trainer` performs exactly the construction sequence of the reference's `main_worker` (train.py:141-207):
-model factory → make_optimizer → convert_syncbn_model → amp.initialize → DDP → loss list; and `step` is the
+model factory → make_optimizer → convert_syncbn_model (+ convert_wsgn_model) → amp.initialize → DDP → loss list; and `step` is the
 loop body: forward, get_total_loss, zero_grad, backward, step, loss mean.  It is what `train.py`, `bench.py`,
 the parity tests and `__graft_entry__.smoke()` all drive, so the measured path is the shipped path.
 """
@@ -16,6 +16,7 @@ from .loss import CEL, BCEWithLogitsLoss, _FusedLossFn, get_total_loss
 from .optim import CustomScheduler, make_optimizer
 from .parallel import DistributedDataParallel
 from .syncbn import convert_syncbn_model
+from .wsgn import convert_wsgn_model
 from .utils import init_seed
 
 # overlap the next batch's host→device copy with the running iteration (see Trainer._stage_inputs).
@@ -46,6 +47,7 @@ class Trainer:
         self.optimizer = make_optimizer(model, optim, dict(lr=lr, momentum=momentum, weight_decay=weight_decay,
                                                            nesterov=nesterov))    # train.py:157
         model = convert_syncbn_model(model)                                # train.py:180 (also at world 1: fused BN)
+        model = convert_wsgn_model(model)                                  # WS-GN backbone: GroupNorm / WS kernels
         self.use_amp = dtype != torch.float32
         if self.use_amp:
             model, self.optimizer = amp.initialize(model, self.optimizer, opt_level="O1", dtype=dtype,

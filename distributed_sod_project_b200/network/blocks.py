@@ -135,13 +135,13 @@ class Bottleneck(nn.Module):
 
     expansion = 4
 
-    def __init__(self, cin: int, width: int, stride: int, shortcut: nn.Module | None):
+    def __init__(self, cin: int, width: int, stride: int, shortcut: nn.Module | None, conv=nn.Conv2d, norm=nn.BatchNorm2d):
         super().__init__()
         cout = width * self.expansion
         specs = ((cin, width, 1, 1, 0), (width, width, 3, stride, 1), (width, cout, 1, 1, 0))
         for i, (ci, co, k, s, p) in enumerate(specs, start=1):
-            setattr(self, f"conv{i}", nn.Conv2d(ci, co, k, s, p, bias=False))
-            setattr(self, f"bn{i}", nn.BatchNorm2d(co))
+            setattr(self, f"conv{i}", conv(ci, co, k, s, p, bias=False))
+            setattr(self, f"bn{i}", norm(co))
         self.relu = nn.ReLU(inplace=True)
         self.downsample = shortcut
         self.stride = stride
@@ -175,15 +175,21 @@ class _StemPool(nn.MaxPool2d):
 _RESNET50_STAGES = ((64, 3, 1), (128, 4, 2), (256, 6, 2), (512, 3, 2))  # (width, blocks, stride)
 
 
-def resnet50_stages() -> tuple[nn.Module, nn.Module, nn.Module, nn.Module, nn.Module]:
+def resnet50_stages(conv=nn.Conv2d, norm=nn.BatchNorm2d, imagenet_fc: bool = False
+                    ) -> tuple[nn.Module, nn.Module, nn.Module, nn.Module, nn.Module]:
     """ResNet-50 encoder sliced into the five strides the decoder taps
     (reference backbone/origin/from_origin.py:7-15): div_2 = stem, div_4 = maxpool+layer1,
     div_8/16/32 = layer2/3/4.  Random init only (no network in this environment; the reference
     would download ImageNet weights, backbone/origin/resnet.py:199-217) — use
     `load_pretrained_backbone` for a local file.
+
+    `conv` / `norm` build every convolution (called as `conv(cin, cout, k, stride, padding, bias=False)`) and every
+    normalisation layer (`norm(channels)`).  `imagenet_fc`: also build (and drop) the 2048→1000 classifier the
+    weight-standardised ResNet constructs before its init loop (backbone/wsgn/resnet.py:105-107), so the random draws
+    after it are the reference's.
     """
-    stem_conv = nn.Conv2d(3, 64, 7, 2, 3, bias=False)
-    stem = _Stem(stem_conv, nn.BatchNorm2d(64), nn.ReLU(inplace=True))
+    stem_conv = conv(3, 64, 7, 2, 3, bias=False)
+    stem = _Stem(stem_conv, norm(64), nn.ReLU(inplace=True))
     pool = _StemPool(3, 2, 1)
 
     layers, cin = [], 64
@@ -195,14 +201,16 @@ def resnet50_stages() -> tuple[nn.Module, nn.Module, nn.Module, nn.Module, nn.Mo
             if b == 0 and (s != 1 or cin != width * Bottleneck.expansion):
                 # built *before* the unit's own convs: keeps the reference's RNG draw order
                 shortcut = nn.Sequential(
-                    nn.Conv2d(cin, width * Bottleneck.expansion, 1, s, bias=False),
-                    nn.BatchNorm2d(width * Bottleneck.expansion),
+                    conv(cin, width * Bottleneck.expansion, 1, s, bias=False),
+                    norm(width * Bottleneck.expansion),
                 )
-            blocks.append(Bottleneck(cin, width, s, shortcut))
+            blocks.append(Bottleneck(cin, width, s, shortcut, conv=conv, norm=norm))
             cin = width * Bottleneck.expansion
         layers.append(nn.Sequential(*blocks))
+    if imagenet_fc:
+        nn.Linear(cin, 1000)
 
-    # He-normal (fan_out) re-init of every conv in module-traversal order, BN γ=1 β=0
+    # He-normal (fan_out) re-init of every conv in module-traversal order, BN γ=1 β=0 (GroupNorm keeps its own 1 / 0)
     for mod in [stem, *layers]:
         for m in mod.modules():
             if isinstance(m, nn.Conv2d):
@@ -211,6 +219,30 @@ def resnet50_stages() -> tuple[nn.Module, nn.Module, nn.Module, nn.Module, nn.Mo
                 nn.init.ones_(m.weight)
                 nn.init.zeros_(m.bias)
     return stem, nn.Sequential(pool, layers[0]), layers[1], layers[2], layers[3]
+
+
+class WSConv2d(nn.Conv2d):
+    """Weight-standardised convolution of the WS-GN backbone (reference backbone/wsgn/customized_func.py:12-25): each
+    filter is centred by the nested means over (C, R, S) and divided by its unbiased std + 1e-5 before the convolution.
+    This is the plain-torch form (CPU, and the stock CUDA model); the engine swaps in `wsgn.FusedWSConv2d`, which runs
+    the same map as one sm_90a kernel per direction.  The amp shadow weights and the optimizer's 16-bit gradient ranges
+    leave these convolutions out: their gradient reaches the fp32 master through the standardisation."""
+
+    eps = 1e-5
+
+    def standardized_weight(self) -> torch.Tensor:
+        w = self.weight
+        w = w - w.mean(dim=1, keepdim=True).mean(dim=2, keepdim=True).mean(dim=3, keepdim=True)
+        std = w.reshape(w.size(0), -1).std(dim=1).view(-1, 1, 1, 1) + self.eps
+        return w / std.expand_as(w)
+
+    def forward(self, x):
+        return self._conv_forward(x, self.standardized_weight(), self.bias)
+
+
+def group_norm32(channels: int) -> nn.GroupNorm:
+    """the WS-GN backbone's `BatchNorm2d` (reference backbone/wsgn/customized_func.py:28-29): GroupNorm(32, C), eps 1e-5"""
+    return nn.GroupNorm(32, channels)
 
 
 class SIM(nn.Module):

@@ -1,4 +1,6 @@
-"""`res50` / `cp_res50`: the TestModel plugin pair of the reference (network/TestModel.py:17-185).
+"""`res50` / `cp_res50`: the TestModel plugin pair of the reference (network/TestModel.py:17-185), and
+`wsgn_res50` / `cp_wsgn_res50`: the same models on the reference's weight-standardised GroupNorm ResNet-50
+(`backbone.wsgn.from_wsgn.Backbone_ResNet50_in3`, the one-import swap in network/TestModel.py:11).
 
 Zero-arg factories looked up by name from `user_config["model"]` (reference train.py:141):
 ResNet-50 encoder → five 1×1 "trans" convs to 64 ch → top-down decoder of SIM + ConvBNReLU with
@@ -14,7 +16,7 @@ import torch
 import torch.nn as nn
 from torch.utils.checkpoint import checkpoint
 
-from .blocks import SIM, ConvBNReLU, bilinear, resnet50_stages, upsample_add
+from .blocks import SIM, ConvBNReLU, WSConv2d, bilinear, group_norm32, resnet50_stages, upsample_add
 
 _TAPS = (32, 16, 8, 4, 2)                       # encoder strides tapped, deepest first
 _TAP_CHANNELS = {32: 2048, 16: 1024, 8: 512, 4: 256, 2: 64}
@@ -22,10 +24,11 @@ _TAP_CHANNELS = {32: 2048, 16: 1024, 8: 512, 4: 256, 2: 64}
 
 class _TestModel(nn.Module):
     recompute = False  # cp_res50 flips this
+    backbone = staticmethod(resnet50_stages)
 
     def __init__(self):
         super().__init__()
-        self.div_2, self.div_4, self.div_8, self.div_16, self.div_32 = resnet50_stages()
+        self.div_2, self.div_4, self.div_8, self.div_16, self.div_32 = self.backbone()
         for s in _TAPS:
             setattr(self, f"trans{s}", nn.Conv2d(_TAP_CHANNELS[s], 64, 1, 1))
         for s in _TAPS:
@@ -79,11 +82,33 @@ class cp_res50(_TestModel):
     recompute = True
 
 
+def _wsgn_backbone():
+    return resnet50_stages(conv=WSConv2d, norm=group_norm32, imagenet_fc=True)
+
+
+class wsgn_res50(_TestModel):
+    """Plain variant on the weight-standardised GroupNorm(32) ResNet-50 (reference backbone/wsgn/from_wsgn.py:8-16):
+    for micro-batch training, where per-GPU batches are too small for BatchNorm.  The decoder keeps BatchNorm."""
+
+    backbone = staticmethod(_wsgn_backbone)
+
+
+class cp_wsgn_res50(wsgn_res50):
+    """Activation-checkpointed twin of `wsgn_res50`, as `cp_res50` is to `res50`."""
+
+    recompute = True
+
+
 def load_pretrained_backbone(model: _TestModel, path: str) -> list[str]:
-    """Load torchvision-format ResNet-50 weights from a local file into `div_*`
-    (the reference downloads them, backbone/origin/resnet.py:199-217; no network here).
-    Keeps the reference's filter-then-update semantics: unknown keys are ignored. Returns loaded keys."""
+    """Load ResNet-50 weights from a local file into `div_*` (the reference downloads them,
+    backbone/origin/resnet.py:199-217 and backbone/wsgn/customized_func.py:32-43; no network here): torchvision's
+    format, or the WS-GN release's — tensors under "state_dict", keys prefixed `module.` (stripped as the reference's
+    `load_pretrained_params` does).  Keeps the reference's filter-then-update semantics: unknown keys are ignored.
+    Returns loaded keys."""
     src = torch.load(path, map_location="cpu")
+    if isinstance(src.get("state_dict"), dict):
+        src = src["state_dict"]
+    src = {k[len("module."):] if k.startswith("module.") else k: v for k, v in src.items()}
     remap = {"conv1.": "div_2.0.", "bn1.": "div_2.1.", "layer1.": "div_4.1.", "layer2.": "div_8.",
              "layer3.": "div_16.", "layer4.": "div_32."}
     own = model.state_dict()

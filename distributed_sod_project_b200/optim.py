@@ -192,6 +192,16 @@ def _same_physical_order(a: torch.Tensor, b: torch.Tensor) -> bool:
     return True
 
 
+def is_plain_conv(m: nn.Module) -> bool:
+    """an nn.Conv2d whose class keeps nn.Conv2d's forward and _conv_forward: the convolution runs on the weight Parameter as
+    it is, so amp may hand it a 16-bit shadow of that weight and the gradient arrives in 16 bit.  A subclass that computes
+    its operand from the weight (the weight-standardised convolutions: network.blocks.WSConv2d, the reference's
+    backbone/wsgn/customized_func.Conv2d) is left alone: a shadow of the raw master would be the wrong operand, and its
+    gradient reaches the fp32 master through the subclass's own computation."""
+    return (isinstance(m, nn.Conv2d) and type(m).forward is nn.Conv2d.forward
+            and type(m)._conv_forward is nn.Conv2d._conv_forward)
+
+
 class FusedOptimizer(Optimizer):
     """What the fused optimizers share: the flat group-major layout (`FlatParams`), the segment table the kernels walk,
     the device learning-rate table, the bf16 gradient gather, `zero_grad`, the shard bounds of world > 1 and the
@@ -204,8 +214,9 @@ class FusedOptimizer(Optimizer):
             raise _lib.SodError(f"at most {_lib.SOD_MAX_SEGMENTS // 2 - 1} parameter groups")
         grouped = {id(p) for g in self.param_groups for p in g["params"]}
         leftovers = [p for p in model.parameters() if id(p) not in grouped] if model is not None else []
-        conv_ids = {id(p) for m in model.modules() if isinstance(m, nn.Conv2d) for p in (m.weight, m.bias) if p is not None} \
-            if model is not None else set()
+        # parameters whose gradient the amp shadow will deliver in 16 bit: those of plain convolutions (amp._install_shadow_weights)
+        conv_ids = {id(p) for m in model.modules() if is_plain_conv(m)
+                    for p in (m.weight, m.bias) if p is not None} if model is not None else set()
         self.flat = FlatParams([list(g["params"]) for g in self.param_groups], leftovers, bf16_grad_ids=conv_ids)
         for p, _ in self.flat.slots:
             flat_registry[id(p)] = self.flat

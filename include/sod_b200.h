@@ -316,6 +316,38 @@ int sod_avgpool2x2_bwd(const void* dy, void* dx, int n, int h_out, int w_out, in
 size_t sod_colsum_workspace_bytes(void);
 int sod_colsum(const void* x, void* out, int64_t rows, int c, int dtype, void* workspace, size_t workspace_bytes, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Weight-standardised GroupNorm ResNet-50 backbone (reference backbone/wsgn/customized_func.py:12-29, resnet.py).
+ *
+ * sod_groupnorm_fwd / _bwd — y = act(GroupNorm(x) [+ residual]) on a channels-last [n·hw, c] matrix, groups ==
+ * SOD_GN_GROUPS, biased variance, fp32 accumulation.  c must be a multiple of groups (else SOD_EINVAL) and a
+ * power-of-two multiple of 8, ≤ 2048 (else SOD_EUNSUPPORTED); x, y, dy, dx, dres, residual and the workspace 16-byte
+ * aligned, save_stats 8-byte aligned (SOD_EALIGN).  save_stats: [n·groups] (mean, rstd) pairs written by the forward
+ * and read by the backward.  The backward reads y for the ReLU mask (relu != 0) and writes dx, dres = masked dy (may be
+ * NULL) and dγ, dβ over the whole batch — added into dgamma / dbeta with SOD_BN_ACCUMULATE_PARAM_GRADS, stored
+ * otherwise.  Deterministic: per-CTA partials merged in fixed order by the last CTA to arrive (integer tickets).
+ * workspace: at least sod_groupnorm_workspace_bytes(n, hw, c, groups) bytes (0 for a shape the kernels refuse),
+ * zero-filled once, then owned by the library (one stream at a time).  sod_groupnorm_splits: the CTAs per sample the
+ * launch uses on the current device (the geometry of oracle/wsgn_geometry.py).
+ *
+ * sod_ws_fwd / _bwd — weight standardisation of `filters` filters of k = C·R·S fp32 weights each (dense per filter,
+ * any memory order): w_hat = (w − μ) / (σ + eps) with the unbiased σ, written once rounded in `dtype`; the backward
+ * takes dw_hat in `dtype` and writes the fp32 dw of that expression (added into dw with
+ * SOD_BN_ACCUMULATE_PARAM_GRADS).  One CTA per filter, deterministic.  k must be > 1.
+ * ------------------------------------------------------------------------------------------------ */
+#define SOD_GN_GROUPS 32
+size_t sod_groupnorm_workspace_bytes(int n, int64_t hw, int c, int groups);
+int sod_groupnorm_splits(int n, int64_t hw, int c, int groups);
+int sod_groupnorm_fwd(const void* x, const void* residual, void* y, int dtype, const float* gamma, const float* beta,
+                      float* save_stats, int n, int64_t hw, int c, int groups, float eps, int relu, void* workspace,
+                      size_t workspace_bytes, void* stream);
+int sod_groupnorm_bwd(const void* dy, const void* x, const void* y, void* dx, void* dres, int dtype, const float* gamma,
+                      const float* save_stats, float* dgamma, float* dbeta, int n, int64_t hw, int c, int groups,
+                      int relu, void* workspace, size_t workspace_bytes, int flags, void* stream);
+int sod_ws_fwd(const float* w, void* w_hat, int dtype, int filters, int k, float eps, void* stream);
+int sod_ws_bwd(const float* w, const void* dw_hat, int dtype, float* dw, int filters, int k, float eps, int flags,
+               void* stream);
+
 /* MaxPool2d(kernel 3, stride 2, padding 1) of the ResNet stem (backbone/origin/resnet.py `maxpool`; `div_4` in
  * backbone/origin/from_origin.py:7-15), channels-last [N,H,W,C], C % 8 == 0; (h, w) = INPUT size, output
  * ((h-1)/2+1, (w-1)/2+1).  argmax: one byte per OUTPUT element (window position kh*3+kw), written by the forward and

@@ -22,6 +22,7 @@ from distributed_sod_project_b200.checkpoint import resume_checkpoint
 from distributed_sod_project_b200.data import open_test_set
 from distributed_sod_project_b200.evaluate import shard, test_process
 from distributed_sod_project_b200.syncbn import convert_syncbn_model
+from distributed_sod_project_b200.wsgn import convert_wsgn_model
 from distributed_sod_project_b200.synthetic import synth_eval_set
 from distributed_sod_project_b200.utils import check_mkdir, construct_exp_name, construct_path_dict, construct_print, write_data_to_file
 
@@ -41,6 +42,7 @@ def main():
     construct_print(f"We will test the model on {world} GPU(s).")
     model = getattr(network, user_config["model"])().cuda().to(memory_format=torch.channels_last)      # reference test.py:40
     model = convert_syncbn_model(model)                        # eval-mode BatchNorm through the same kernels as training
+    model = convert_wsgn_model(model)                          # and the WS-GN backbone's GroupNorm / WS kernels
     resume_checkpoint(model=model, load_path=path_config["final_full_net"], mode="onlynet", local_rank=local)
     total_results = {}
     if not user_config.get("synthetic_eval", True):

@@ -190,7 +190,7 @@ def step_vectors(model_name: str, world: int, bs: int, size: int, iters: int, ta
     np.savez_compressed(os.path.join(OUT, f"step_{tag}.npz"), **out)
 
 
-def model_init_vectors(model_name: str = "res50", samples: int = 32):
+def model_init_vectors(model_name: str = "res50", samples: int = 32, tag: str | None = None):
     """the reference model right after `init_seed(0)`: every state_dict key and shape, per-tensor float64 sum and sum of
     squares, a fixed seeded sample of values per tensor, and the output of one forward pass on a seeded input
     (tests/test_host_cpu.py::test_model_plugin_is_bit_identical_to_reference compares the package's plugin with it)"""
@@ -209,7 +209,7 @@ def model_init_vectors(model_name: str = "res50", samples: int = 32):
     x = torch.randn(2, 3, 64, 64, generator=torch.Generator().manual_seed(0))
     out = {"keys": np.array("\n".join(sd)), "shapes": np.array(shapes, dtype=np.int64), "values": np.array(vals),
            "moments": np.array(moments), "x": x.numpy(), "y": model(x).detach().numpy()}
-    np.savez_compressed(os.path.join(OUT, f"model_{model_name}_init.npz"), **out)
+    np.savez_compressed(os.path.join(OUT, f"model_{tag or model_name}_init.npz"), **out)
 
 
 def main():
