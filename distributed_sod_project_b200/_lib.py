@@ -27,6 +27,7 @@ SOD_BN_LAUNCH_COOP = 128
 SOD_BN_LAUNCH_PDL = 256
 SOD_GRAD16_F16 = 512
 SOD_GN_GROUPS = 32
+SOD_GCONV_GROUPS = 32
 SOD_RESIZE_BILINEAR = 2
 SOD_RESIZE_BICUBIC = 3
 SOD_GATHER_MAX_ITEMS = 160
@@ -164,6 +165,14 @@ _PROTOTYPES = {
                                     C.c_int, C.c_void_p]),
     "sod_ws_fwd": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_float, C.c_void_p]),
     "sod_ws_bwd": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_float, C.c_int, C.c_void_p]),
+    "sod_gconv3x3_fwd": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+                                   C.c_int, C.c_void_p]),
+    "sod_gconv3x3_dgrad": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+                                     C.c_int, C.c_void_p]),
+    "sod_gconv3x3_wgrad_splits": (C.c_int, [C.c_int] * 6),
+    "sod_gconv3x3_wgrad_workspace_bytes": (C.c_size_t, [C.c_int] * 6),
+    "sod_gconv3x3_wgrad": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+                                     C.c_int, C.c_void_p, C.c_size_t, C.c_void_p]),
 }
 
 EXPORTS = tuple(_PROTOTYPES)

@@ -19,6 +19,8 @@ torch elementwise kernels.  On a stock `nn.BatchNorm2d` the same helper runs pla
 """
 from __future__ import annotations
 
+import math
+
 import torch
 import torch.nn as nn
 import torch.nn.functional as F
@@ -131,16 +133,22 @@ class ConvBNReLU(nn.Module):
 
 class Bottleneck(nn.Module):
     """1x1 → 3x3(stride) → 1x1(×4) residual unit with the torchvision-v1 naming
-    (`conv1,bn1,conv2,bn2,conv3,bn3,relu,downsample`), stride on the 3x3."""
+    (`conv1,bn1,conv2,bn2,conv3,bn3,relu,downsample`), stride on the 3x3.
+
+    With `cardinality` C > 1 it is the ResNeXt unit of the reference (backbone/wsgn/resnext.py:21-52): the inner width
+    is D·C with D = floor(planes·base_width / 64), and the 3x3 is a C-group convolution."""
 
     expansion = 4
 
-    def __init__(self, cin: int, width: int, stride: int, shortcut: nn.Module | None, conv=nn.Conv2d, norm=nn.BatchNorm2d):
+    def __init__(self, cin: int, planes: int, stride: int, shortcut: nn.Module | None, conv=nn.Conv2d,
+                 norm=nn.BatchNorm2d, cardinality: int = 1, base_width: int = 64):
         super().__init__()
-        cout = width * self.expansion
-        specs = ((cin, width, 1, 1, 0), (width, width, 3, stride, 1), (width, cout, 1, 1, 0))
-        for i, (ci, co, k, s, p) in enumerate(specs, start=1):
-            setattr(self, f"conv{i}", conv(ci, co, k, s, p, bias=False))
+        width = int(math.floor(planes * (base_width / 64))) * cardinality
+        cout = planes * self.expansion
+        specs = ((cin, width, 1, 1, 0, 1), (width, width, 3, stride, 1, cardinality), (width, cout, 1, 1, 0, 1))
+        for i, (ci, co, k, s, p, g) in enumerate(specs, start=1):
+            setattr(self, f"conv{i}", conv(ci, co, k, s, p, bias=False) if g == 1 else
+                    conv(ci, co, k, s, p, groups=g, bias=False))
             setattr(self, f"bn{i}", norm(co))
         self.relu = nn.ReLU(inplace=True)
         self.downsample = shortcut
@@ -175,8 +183,8 @@ class _StemPool(nn.MaxPool2d):
 _RESNET50_STAGES = ((64, 3, 1), (128, 4, 2), (256, 6, 2), (512, 3, 2))  # (width, blocks, stride)
 
 
-def resnet50_stages(conv=nn.Conv2d, norm=nn.BatchNorm2d, imagenet_fc: bool = False
-                    ) -> tuple[nn.Module, nn.Module, nn.Module, nn.Module, nn.Module]:
+def resnet50_stages(conv=nn.Conv2d, norm=nn.BatchNorm2d, imagenet_fc: bool = False, cardinality: int = 1,
+                    base_width: int = 64) -> tuple[nn.Module, nn.Module, nn.Module, nn.Module, nn.Module]:
     """ResNet-50 encoder sliced into the five strides the decoder taps
     (reference backbone/origin/from_origin.py:7-15): div_2 = stem, div_4 = maxpool+layer1,
     div_8/16/32 = layer2/3/4.  Random init only (no network in this environment; the reference
@@ -187,6 +195,10 @@ def resnet50_stages(conv=nn.Conv2d, norm=nn.BatchNorm2d, imagenet_fc: bool = Fal
     normalisation layer (`norm(channels)`).  `imagenet_fc`: also build (and drop) the 2048→1000 classifier the
     weight-standardised ResNet constructs before its init loop (backbone/wsgn/resnet.py:105-107), so the random draws
     after it are the reference's.
+
+    `cardinality` > 1 builds ResNeXt-50 (cardinality × base_width d) instead, with the reference ResNeXt's init
+    expression `normal_(0, math.sqrt(2.0 / n))`, n = k·k·out_channels (backbone/wsgn/resnext.py:109-112).  It is the
+    same distribution as He-normal fan_out, but for some n `sqrt(2/n)` and `sqrt(2)/sqrt(n)` differ in the last bit.
     """
     stem_conv = conv(3, 64, 7, 2, 3, bias=False)
     stem = _Stem(stem_conv, norm(64), nn.ReLU(inplace=True))
@@ -204,7 +216,8 @@ def resnet50_stages(conv=nn.Conv2d, norm=nn.BatchNorm2d, imagenet_fc: bool = Fal
                     conv(cin, width * Bottleneck.expansion, 1, s, bias=False),
                     norm(width * Bottleneck.expansion),
                 )
-            blocks.append(Bottleneck(cin, width, s, shortcut, conv=conv, norm=norm))
+            blocks.append(Bottleneck(cin, width, s, shortcut, conv=conv, norm=norm, cardinality=cardinality,
+                                     base_width=base_width))
             cin = width * Bottleneck.expansion
         layers.append(nn.Sequential(*blocks))
     if imagenet_fc:
@@ -213,7 +226,11 @@ def resnet50_stages(conv=nn.Conv2d, norm=nn.BatchNorm2d, imagenet_fc: bool = Fal
     # He-normal (fan_out) re-init of every conv in module-traversal order, BN γ=1 β=0 (GroupNorm keeps its own 1 / 0)
     for mod in [stem, *layers]:
         for m in mod.modules():
-            if isinstance(m, nn.Conv2d):
+            if isinstance(m, nn.Conv2d) and cardinality > 1:
+                n = m.kernel_size[0] * m.kernel_size[1] * m.out_channels
+                with torch.no_grad():
+                    m.weight.normal_(0, math.sqrt(2.0 / n))
+            elif isinstance(m, nn.Conv2d):
                 nn.init.kaiming_normal_(m.weight, mode="fan_out", nonlinearity="relu")
             elif isinstance(m, nn.BatchNorm2d):
                 nn.init.ones_(m.weight)

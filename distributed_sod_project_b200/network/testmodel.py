@@ -1,6 +1,9 @@
 """`res50` / `cp_res50`: the TestModel plugin pair of the reference (network/TestModel.py:17-185), and
 `wsgn_res50` / `cp_wsgn_res50`: the same models on the reference's weight-standardised GroupNorm ResNet-50
-(`backbone.wsgn.from_wsgn.Backbone_ResNet50_in3`, the one-import swap in network/TestModel.py:11).
+(`backbone.wsgn.from_wsgn.Backbone_ResNet50_in3`, the one-import swap in network/TestModel.py:11), and
+`wsgn_resnext50` / `cp_wsgn_resnext50`: the same on its weight-standardised GroupNorm ResNeXt-50 32×4d
+(`Backbone_ResNeXt50_in3`, built as `l_resnext50(pretrained, baseWidth=4, cardinality=32)`: the reference's builder
+omits those two arguments, and its X-50-GN-WS release is 32×4d).
 
 Zero-arg factories looked up by name from `user_config["model"]` (reference train.py:141):
 ResNet-50 encoder → five 1×1 "trans" convs to 64 ch → top-down decoder of SIM + ConvBNReLU with
@@ -95,6 +98,23 @@ class wsgn_res50(_TestModel):
 
 class cp_wsgn_res50(wsgn_res50):
     """Activation-checkpointed twin of `wsgn_res50`, as `cp_res50` is to `res50`."""
+
+    recompute = True
+
+
+def _wsgn_resnext_backbone():
+    return resnet50_stages(conv=WSConv2d, norm=group_norm32, imagenet_fc=True, cardinality=32, base_width=4)
+
+
+class wsgn_resnext50(_TestModel):
+    """Plain variant on the weight-standardised GroupNorm(32) ResNeXt-50 32×4d (reference
+    backbone/wsgn/from_wsgn.py:19-27, resnext.py): every bottleneck's 3x3 is a 32-group convolution."""
+
+    backbone = staticmethod(_wsgn_resnext_backbone)
+
+
+class cp_wsgn_resnext50(wsgn_resnext50):
+    """Activation-checkpointed twin of `wsgn_resnext50`."""
 
     recompute = True
 

@@ -6,7 +6,10 @@
   per direction (the model's `bn_act` drives it unchanged);
 * every `network.blocks.WSConv2d` for `FusedWSConv2d`, which standardises its fp32 master weight with one kernel per
   direction and hands the convolution Ŵ in the convolution's dtype (under autocast: rounded once from fp32, as apex O1
-  standardises in fp32 and casts afterwards).
+  standardises in fp32 and casts afterwards).  The ResNeXt backbone's 32-group 3×3 convolutions run on the
+  csrc/gconv.cu kernels where those measured faster than cuDNN (`grouped_conv_on_kernels`), their fp32 weight
+  gradient going straight into the standardisation's backward, and on cuDNN elsewhere; a grouped WS convolution outside
+  the kernels' geometry raises SodError.
 The swapped modules SHARE the original Parameter objects, so an optimizer built before the conversion keeps training
 them.  Models without GroupNorm or WS convolutions come back untouched.  There is no CPU or torch fallback: a CPU tensor
 or a shape the kernels do not cover raises SodError.
@@ -22,16 +25,17 @@ import torch.nn as nn
 from . import _lib
 from .network.blocks import WSConv2d
 
-# one workspace per device, grown when a larger shape arrives; outgrown buffers are kept alive because a captured CUDA
-# graph may still hold their address
+# one workspace per device and user ("groupnorm": zero-filled tickets the kernels keep at zero; "gconv": the grouped
+# convolutions' wgrad partials), grown when a larger shape arrives; outgrown buffers are kept alive because a captured
+# CUDA graph may still hold their address
 _workspaces: dict = {}
 
 
-def _workspace(device: torch.device, nbytes: int) -> torch.Tensor:
-    bufs = _workspaces.setdefault(device.index, [])
+def _workspace(device: torch.device, nbytes: int, user: str = "groupnorm") -> torch.Tensor:
+    bufs = _workspaces.setdefault((device.index, user), [])
     if not bufs or bufs[-1].numel() < nbytes:
         if torch.cuda.is_current_stream_capturing():
-            raise _lib.SodError(f"GroupNorm workspace of {nbytes} bytes needed while a CUDA graph is being captured; "
+            raise _lib.SodError(f"{user} workspace of {nbytes} bytes needed while a CUDA graph is being captured; "
                                 "run the shape eagerly once first")
         bufs.append(torch.zeros(max(nbytes, 1 << 20), dtype=torch.uint8, device=device))
     return bufs[-1]
@@ -171,13 +175,91 @@ def standardize_weight(weight: torch.Tensor, dtype: torch.dtype, eps: float = 1e
     return _WSFn.apply(weight, dtype, eps)
 
 
+class _WSGroupConvFn(torch.autograd.Function):
+    """y = conv3x3(x, WS(weight), groups=32, padding 1, stride s) on csrc/gconv.cu; the backward hands the fp32 dŴ of
+    the wgrad kernel to sod_ws_bwd unrounded (an autograd edge between two Functions would round it to Ŵ's dtype)"""
+
+    @staticmethod
+    def forward(ctx, x, weight, dtype, eps, stride):
+        x = _as_rows(x).to(dtype)
+        n, c, h, w = x.shape
+        w_hat = torch.empty_like(weight, dtype=dtype)              # the master's memory order
+        rc = _lib.lib().sod_ws_fwd(weight.data_ptr(), w_hat.data_ptr(), _lib.dtype_code(dtype), weight.shape[0],
+                                   weight[0].numel(), float(eps), _lib.stream_ptr())
+        _lib.check(rc, "sod_ws_fwd")
+        w_hat = _as_rows(w_hat)                                    # [C_out][3][3][C_in / 32], the kernels' order
+        y = torch.empty((n, c, (h - 1) // stride + 1, (w - 1) // stride + 1), dtype=dtype, device=x.device,
+                        memory_format=torch.channels_last)
+        rc = _lib.lib().sod_gconv3x3_fwd(x.data_ptr(), w_hat.data_ptr(), y.data_ptr(), _lib.dtype_code(dtype), n, h, w,
+                                         c, _lib.SOD_GCONV_GROUPS, stride, _lib.stream_ptr())
+        _lib.check(rc, "sod_gconv3x3_fwd")
+        _lib.count_launch(2)
+        ctx.eps, ctx.stride, ctx.weight_ref = eps, stride, weight
+        ctx.save_for_backward(x, weight, w_hat)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        x, weight, w_hat = ctx.saved_tensors
+        n, c, h, w = x.shape
+        dy = _as_rows(dy).to(x.dtype)
+        code, G, s, lib = _lib.dtype_code(x.dtype), _lib.SOD_GCONV_GROUPS, ctx.stride, _lib.lib()
+        dx = torch.empty_like(x)
+        _lib.check(lib.sod_gconv3x3_dgrad(dy.data_ptr(), w_hat.data_ptr(), dx.data_ptr(), code, n, h, w, c, G, s,
+                                          _lib.stream_ptr()), "sod_gconv3x3_dgrad")
+        dw_hat = torch.empty(weight.shape, dtype=torch.float32, device=x.device, memory_format=torch.channels_last)
+        ws = _workspace(x.device, int(lib.sod_gconv3x3_wgrad_workspace_bytes(n, h, w, c, G, s)), "gconv")
+        _lib.check(lib.sod_gconv3x3_wgrad(x.data_ptr(), dy.data_ptr(), dw_hat.data_ptr(), code, n, h, w, c, G, s,
+                                          ws.data_ptr(), ws.numel(), _lib.stream_ptr()), "sod_gconv3x3_wgrad")
+        if dw_hat.stride() != weight.stride():
+            dw_hat = torch.empty_like(weight, dtype=torch.float32).copy_(dw_hat)
+        bound = _bound_fp32_grad(ctx.weight_ref)
+        if bound is not None:
+            dw, flags = bound, _lib.SOD_BN_ACCUMULATE_PARAM_GRADS
+            _lib.grad_writes += 1
+        else:
+            dw, flags = torch.empty_like(weight, dtype=torch.float32), 0
+        _lib.check(lib.sod_ws_bwd(weight.data_ptr(), dw_hat.data_ptr(), _lib.SOD_F32, dw.data_ptr(), weight.shape[0],
+                                  weight[0].numel(), float(ctx.eps), flags, _lib.stream_ptr()), "sod_ws_bwd")
+        _lib.count_launch(4)
+        return dx, (None if bound is not None else dw.to(weight.dtype)), None, None, None
+
+
+def grouped_conv_covered(conv: nn.Conv2d) -> bool:
+    """the geometry of csrc/gconv.cu: 32 groups of 4, 8, 16 or 32 channels, C_in = C_out, 3×3, padding 1, dilation 1,
+    stride 1 or 2, no bias"""
+    cpg = conv.in_channels // conv.groups
+    return (conv.groups == _lib.SOD_GCONV_GROUPS and conv.in_channels == conv.out_channels and cpg in (4, 8, 16, 32)
+            and conv.kernel_size == (3, 3) and conv.padding == (1, 1) and conv.dilation == (1, 1)
+            and conv.stride in ((1, 1), (2, 2)) and conv.bias is None and conv.padding_mode == "zeros")
+
+
+def grouped_conv_on_kernels(conv: nn.Conv2d) -> bool:
+    """which covered grouped convolutions run on csrc/gconv.cu rather than cuDNN: measured per shape on an H100
+    (DESIGN §4.13, tools/bench_wsgn.py --model wsgn_resnext50), fwd + dgrad + wgrad of the kernels beat cuDNN only at
+    8 channels per group and stride 2 (layer2.0), where cuDNN's dgrad is 3.6× slower; at every other shape of the
+    backbone cuDNN's grouped kernels are 1.3–8.5× faster than these"""
+    return conv.in_channels // conv.groups == 8 and conv.stride == (2, 2)
+
+
 class FusedWSConv2d(WSConv2d):
-    """Drop-in for `WSConv2d` that `convert_wsgn_model` installs: the standardisation runs as sm_90a kernels."""
+    """Drop-in for `WSConv2d` that `convert_wsgn_model` installs: the standardisation runs as sm_90a kernels, and so
+    does a 32-group 3×3 convolution where they beat cuDNN (`grouped_conv_on_kernels`)."""
 
     def forward(self, x):
         if not x.is_cuda:
             raise _lib.SodError("FusedWSConv2d: expected a CUDA tensor (keep network.blocks.WSConv2d for CPU runs)")
         dtype = torch.get_autocast_dtype("cuda") if torch.is_autocast_enabled("cuda") else self.weight.dtype
+        if self.groups != 1:
+            if not grouped_conv_covered(self) or x.dim() != 4 or self.weight.dtype != torch.float32:
+                raise _lib.SodError(
+                    f"FusedWSConv2d: the grouped-convolution kernels do not cover groups={self.groups}, "
+                    f"{self.in_channels}->{self.out_channels} channels, kernel {self.kernel_size}, stride {self.stride}, "
+                    f"padding {self.padding}, dilation {self.dilation}, bias={self.bias is not None}, "
+                    f"{x.dim()}-D {x.dtype} input, {self.weight.dtype} weight (32 groups of 4/8/16/32 channels, 3x3, "
+                    "padding 1, stride 1 or 2, no bias, fp32 master weight)")
+            if grouped_conv_on_kernels(self):
+                return _WSGroupConvFn.apply(x, self.weight, dtype, self.eps, self.stride[0])
         return self._conv_forward(x, standardize_weight(self.weight, dtype, self.eps), self.bias)
 
 

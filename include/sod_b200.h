@@ -348,6 +348,32 @@ int sod_ws_fwd(const float* w, void* w_hat, int dtype, int filters, int k, float
 int sod_ws_bwd(const float* w, const void* dw_hat, int dtype, float* dw, int filters, int k, float eps, int flags,
                void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * 32-group 3×3 convolutions of the weight-standardised GroupNorm ResNeXt-50 32×4d backbone (reference
+ * backbone/wsgn/resnext.py `conv2`): padding 1, dilation 1, no bias, C_in = C_out = c, groups == SOD_GCONV_GROUPS,
+ * c / groups ∈ {4, 8, 16, 32}, stride 1 or 2, any h, w ≥ 1 (else SOD_EUNSUPPORTED; c not a multiple of groups, a bad
+ * dtype or a non-positive size is SOD_EINVAL).  Activations channels-last [n, h, w, c] / [n, ho, wo, c] with
+ * ho = (h − 1) / stride + 1 (likewise wo) in `dtype`; (h, w) is the size of x in every entry.  w_hat is
+ * [c][3][3][c / groups] in `dtype` (a channels-last weight's memory order); the weight gradient dw_hat is fp32 in the
+ * same order (what sod_ws_bwd reads with dtype SOD_F32).  fp32 accumulation; fp32 activations are computed in fp32
+ * (no TF32), 16-bit ones on tensor cores.  Every pointer 16-byte aligned (SOD_EALIGN).
+ *
+ * sod_gconv3x3_fwd: y from x.  sod_gconv3x3_dgrad: dx from dy (the transposed convolution).
+ * sod_gconv3x3_wgrad: dw_hat from x and dy, stored (not accumulated).  The pixels are split into
+ * sod_gconv3x3_wgrad_splits(...) fixed chunks (oracle/gconv_geometry.py; a function of the shape only), whose fp32
+ * partials go to the workspace — at least sod_gconv3x3_wgrad_workspace_bytes(...) bytes, 0 for a refused shape — and
+ * are added in chunk order by a second launch.  Deterministic; no refusal launches anything.
+ * ------------------------------------------------------------------------------------------------ */
+#define SOD_GCONV_GROUPS 32
+int sod_gconv3x3_fwd(const void* x, const void* w_hat, void* y, int dtype, int n, int h, int w, int c, int groups,
+                     int stride, void* stream);
+int sod_gconv3x3_dgrad(const void* dy, const void* w_hat, void* dx, int dtype, int n, int h, int w, int c, int groups,
+                       int stride, void* stream);
+int sod_gconv3x3_wgrad_splits(int n, int h, int w, int c, int groups, int stride);
+size_t sod_gconv3x3_wgrad_workspace_bytes(int n, int h, int w, int c, int groups, int stride);
+int sod_gconv3x3_wgrad(const void* x, const void* dy, float* dw_hat, int dtype, int n, int h, int w, int c, int groups,
+                       int stride, void* workspace, size_t workspace_bytes, void* stream);
+
 /* MaxPool2d(kernel 3, stride 2, padding 1) of the ResNet stem (backbone/origin/resnet.py `maxpool`; `div_4` in
  * backbone/origin/from_origin.py:7-15), channels-last [N,H,W,C], C % 8 == 0; (h, w) = INPUT size, output
  * ((h-1)/2+1, (w-1)/2+1).  argmax: one byte per OUTPUT element (window position kh*3+kw), written by the forward and

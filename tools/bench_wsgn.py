@@ -1,9 +1,9 @@
 #!/usr/bin/env python
 """Measure the WS-GN backbone on the GPU; one JSON line on stdout.
 
-    python tools/bench_wsgn.py [--steps K --warmup W]
+    python tools/bench_wsgn.py [--model wsgn_res50 | wsgn_resnext50] [--steps K --warmup W]
 
-On the bench workload (320×320, bs 16, bf16):
+On the bench workload (320×320, bs 16, bf16), `--model wsgn_res50` (the default):
 * `wsgn_res50`: images/s of the engine's iteration (GroupNorm / WS kernels, SyncBN decoder, fused loss and SGD),
   replayed from a CUDA graph, batch resident in HBM;
 * `stock`: the same model in stock PyTorch — the reference's WS expression, nn.GroupNorm, nn.BatchNorm2d, channels-last,
@@ -14,6 +14,13 @@ On the bench workload (320×320, bs 16, bf16):
   algorithmic GB/s (bytes the algorithm has to move: the kernels read x and write y forward, read dy, x, y and write dx
   backward; torch reads x, writes y forward and reads dy, x and writes dx backward);
 * `ws_us`: weight standardisation forward + backward of all 53 convolutions of the model, device µs from a CUDA graph.
+`--model wsgn_resnext50`:
+* images/s of the engine's iteration and of the stock eager model, as above, on the ResNeXt-50 32×4d backbone;
+* `gconv`: per distinct shape of its sixteen 32-group 3×3 convolutions, fwd, dgrad and wgrad µs of the csrc/gconv.cu
+  entries and of cuDNN (`F.conv2d(groups=32)` and `aten.convolution_backward`, cudnn.benchmark on) on the same
+  channels-last bf16 tensors, each device time from a CUDA graph of back-to-back calls, with achieved TFLOP/s
+  (2·Ho·Wo·N·C·9·cpg per direction) and algorithmic GB/s (fwd reads x, Ŵ and writes y; dgrad reads dy, Ŵ and writes
+  dx; wgrad reads x, dy and writes dŴ — fp32 for the kernels, bf16 for cuDNN).
 The card's name and power limit are part of the line.
 """
 from __future__ import annotations
@@ -31,6 +38,9 @@ import torch  # noqa: E402
 import torch.nn.functional as F  # noqa: E402
 
 SIZE, BS = 320, 16
+# (C, channels per group, stride, input side) of the ResNeXt backbone's grouped 3×3 convolutions at a 320×320 input
+GCONV_SHAPES = ((128, 4, 1, 80), (256, 8, 2, 80), (256, 8, 1, 40), (512, 16, 2, 40), (512, 16, 1, 20),
+                (1024, 32, 2, 20), (1024, 32, 1, 10))
 # (channels, side) of the backbone's GroupNorm layers at a 320×320 input
 GN_SHAPES = ((64, 160), (64, 80), (128, 80), (256, 80), (128, 40), (256, 40), (512, 40), (256, 20), (512, 20),
              (1024, 20), (512, 10), (2048, 10))
@@ -52,10 +62,10 @@ def timed_ms(fn, iters: int) -> float:
     return a.elapsed_time(b) / iters
 
 
-def engine_img_s(steps: int, warmup: int) -> float:
+def engine_img_s(steps: int, warmup: int, model_name: str = "wsgn_res50") -> float:
     from distributed_sod_project_b200.engine import Trainer
     from distributed_sod_project_b200.synthetic import synth_batch
-    tr = Trainer(model_name="wsgn_res50", dtype=torch.bfloat16, use_graph=True, report_items=False)
+    tr = Trainer(model_name=model_name, dtype=torch.bfloat16, use_graph=True, report_items=False)
     x, m = (t.cuda() for t in synth_batch(0, BS, SIZE))
     for _ in range(warmup):
         tr.forward_backward_update(x, m, report=False)
@@ -63,12 +73,12 @@ def engine_img_s(steps: int, warmup: int) -> float:
     return BS / (timed_ms(lambda: tr.forward_backward_update(x, m, report=False), steps) * 1e-3)
 
 
-def stock_img_s(steps: int, warmup: int) -> float:
+def stock_img_s(steps: int, warmup: int, model_name: str = "wsgn_res50") -> float:
     from distributed_sod_project_b200 import network
     from distributed_sod_project_b200.synthetic import synth_batch
     from distributed_sod_project_b200.utils import init_seed
     init_seed(0)
-    model = network.wsgn_res50().cuda().to(memory_format=torch.channels_last).train()
+    model = getattr(network, model_name)().cuda().to(memory_format=torch.channels_last).train()
     opt = torch.optim.SGD(model.parameters(), lr=0.05, momentum=0.9, weight_decay=5e-4)
     x, m = (t.cuda() for t in synth_batch(0, BS, SIZE))
     x = x.contiguous(memory_format=torch.channels_last)
@@ -171,17 +181,73 @@ def ws_model_us() -> float:
     return round(graph_us(both, reps=2, replays=20), 1)
 
 
+def gconv_flops_bytes(c: int, cpg: int, stride: int, side: int, es: int = 2) -> dict:
+    """operations of one direction, and the bytes each direction has to move, from the shape"""
+    so = (side - 1) // stride + 1
+    x, y, w = BS * side * side * c * es, BS * so * so * c * es, c * 9 * cpg
+    return {"flop": 2 * BS * so * so * c * 9 * cpg, "fwd": x + w * es + y, "dgrad": y + w * es + x,
+            "wgrad_sod": x + y + 4 * w, "wgrad_cudnn": x + y + w * es}
+
+
+def gconv_layers() -> list[dict]:
+    from distributed_sod_project_b200 import _lib
+    lib, G, st = _lib.lib(), _lib.SOD_GCONV_GROUPS, _lib.stream_ptr
+    torch.backends.cudnn.benchmark = True
+    rows = []
+    for c, cpg, stride, side in GCONV_SHAPES:
+        g = torch.Generator(device="cuda").manual_seed(c + side)
+        cl, so = torch.channels_last, (side - 1) // stride + 1
+        x = torch.randn(BS, c, side, side, device="cuda", generator=g).to(torch.bfloat16).contiguous(memory_format=cl)
+        dy = torch.randn(BS, c, so, so, device="cuda", generator=g).to(torch.bfloat16).contiguous(memory_format=cl)
+        w = (torch.randn(c, cpg, 3, 3, device="cuda", generator=g) * 0.1).to(torch.bfloat16).contiguous(memory_format=cl)
+        y, dx = torch.empty_like(dy), torch.empty_like(x)
+        dw = torch.empty(w.shape, dtype=torch.float32, device="cuda", memory_format=cl)
+        ws = torch.empty(int(lib.sod_gconv3x3_wgrad_workspace_bytes(BS, side, side, c, G, stride)), dtype=torch.uint8,
+                         device="cuda")
+        bf16 = _lib.dtype_code(x.dtype)
+        sod = {
+            "fwd": lambda: _lib.check(lib.sod_gconv3x3_fwd(x.data_ptr(), w.data_ptr(), y.data_ptr(), bf16, BS, side,
+                                                           side, c, G, stride, st())),
+            "dgrad": lambda: _lib.check(lib.sod_gconv3x3_dgrad(dy.data_ptr(), w.data_ptr(), dx.data_ptr(), bf16, BS,
+                                                               side, side, c, G, stride, st())),
+            "wgrad": lambda: _lib.check(lib.sod_gconv3x3_wgrad(x.data_ptr(), dy.data_ptr(), dw.data_ptr(), bf16, BS,
+                                                               side, side, c, G, stride, ws.data_ptr(), ws.numel(),
+                                                               st())),
+        }
+        cb = torch.ops.aten.convolution_backward
+        cudnn = {
+            "fwd": lambda: F.conv2d(x, w, None, stride, 1, 1, G),
+            "dgrad": lambda: cb(dy, x, w, None, [stride] * 2, [1, 1], [1, 1], False, [0, 0], G, [True, False, False]),
+            "wgrad": lambda: cb(dy, x, w, None, [stride] * 2, [1, 1], [1, 1], False, [0, 0], G, [False, True, False]),
+        }
+        fb = gconv_flops_bytes(c, cpg, stride, side)
+        out = {"c": c, "cpg": cpg, "stride": stride, "hw": side, "n": BS}
+        for name, fns in (("sod", sod), ("cudnn", cudnn)):
+            for d, fn in fns.items():
+                t = graph_us(fn)
+                nbytes = fb[d] if d != "wgrad" else fb[f"wgrad_{name}"]
+                out[f"{name}_{d}_us"] = round(t, 2)
+                out[f"{name}_{d}_tflops"] = round(fb["flop"] / (t * 1e-6) / 1e12, 2)
+                out[f"{name}_{d}_gbs"] = round(nbytes / (t * 1e-6) / 1e9, 1)
+        rows.append(out)
+    return rows
+
+
 def main():
     ap = argparse.ArgumentParser()
+    ap.add_argument("--model", choices=("wsgn_res50", "wsgn_resnext50"), default="wsgn_res50")
     ap.add_argument("--steps", type=int, default=30)
     ap.add_argument("--warmup", type=int, default=5)
     args = ap.parse_args()
     torch.cuda.set_device(0)
     line = {"gpu": card(), "workload": f"{SIZE}x{SIZE}, bs {BS}, bf16"}
-    line["wsgn_res50_img_s"] = round(engine_img_s(args.steps, args.warmup), 1)
-    line["stock_img_s"] = round(stock_img_s(args.steps, args.warmup), 1)
-    line["groupnorm"] = groupnorm_layers()
-    line["ws_us"] = ws_model_us()
+    line[f"{args.model}_img_s"] = round(engine_img_s(args.steps, args.warmup, args.model), 1)
+    line["stock_img_s"] = round(stock_img_s(args.steps, args.warmup, args.model), 1)
+    if args.model == "wsgn_res50":
+        line["groupnorm"] = groupnorm_layers()
+        line["ws_us"] = ws_model_us()
+    else:
+        line["gconv"] = gconv_layers()
     print(json.dumps(line), flush=True)
 
 
