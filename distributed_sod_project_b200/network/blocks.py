@@ -1,4 +1,4 @@
-"""Building blocks of the TestModel plugin family (`res50`, `cp_res50`).
+"""Building blocks of the TestModel plugin family (`res50`, `cp_res50`, and their WS-GN and VGG16-BN variants).
 
 Written from scratch for this repo; the *contract* it keeps is the reference's
 (lartpang/Distributed-SOD-Project):
@@ -236,6 +236,54 @@ def resnet50_stages(conv=nn.Conv2d, norm=nn.BatchNorm2d, imagenet_fc: bool = Fal
                 nn.init.ones_(m.weight)
                 nn.init.zeros_(m.bias)
     return stem, nn.Sequential(pool, layers[0]), layers[1], layers[2], layers[3]
+
+
+class _VGGPool(nn.MaxPool2d):
+    """VGG16-BN's MaxPool2d(2, 2); routed to csrc/maxpool.cu when that kernel is enabled (the default)"""
+
+    def forward(self, x):
+        from .. import resample
+        cover = (self.kernel_size, self.stride, self.padding, self.dilation, self.ceil_mode) == (2, 2, 0, 1, False)
+        y = resample.maxpool2x2s2(x) if cover and not self.return_indices else None
+        return y if y is not None else super().forward(x)
+
+
+class _VGGSlice(nn.Sequential):
+    """A slice of VGG16-BN's `features`, indexed from 0 as the reference's `nn.Sequential(*features[a:b])` is.  Each
+    conv → BN → ReLU triple runs as `conv_bn_act`, so the engine folds the convolution's bias into the SyncBN kernel."""
+
+    def forward(self, x):
+        mods = list(self)
+        i = 0
+        while i < len(mods):
+            if isinstance(mods[i], nn.Conv2d):
+                x = conv_bn_act(mods[i], mods[i + 1], x)
+                i += 3
+            else:
+                x = mods[i](x)
+                i += 1
+        return x
+
+
+_VGG16_CFG = (64, 64, "M", 128, 128, "M", 256, 256, 256, "M", 512, 512, 512, "M", 512, 512, 512)   # "D", last "M" dropped
+VGG16_SLICES = ((0, 6), (6, 13), (13, 23), (23, 33), (33, 43))    # features[a:b] of each of the five slices
+
+
+def vgg16_bn_slices() -> tuple[nn.Module, nn.Module, nn.Module, nn.Module, nn.Module]:
+    """VGG16-BN's `features` cut into the five slices the decoder taps (reference backbone/origin/from_origin.py:18-25):
+    two conv–BN–ReLU triples at full resolution, then four slices that each open with a 2×2 max-pool.  The fifth pool
+    (features[43]) is not part of the backbone.  Modules are built in `make_layers` order (backbone/origin/vgg.py) and
+    nothing is re-initialised: the reference builds with `pretrained=True`, which passes `init_weights=False`, so its
+    convolutions keep torch's default init (kaiming-uniform weights, uniform biases) and its BatchNorms 1 / 0.  Random init
+    only (no network here) — use `load_pretrained_backbone` for torchvision's `vgg16_bn` file."""
+    layers, cin = [], 3
+    for v in _VGG16_CFG:
+        if v == "M":
+            layers.append(_VGGPool(2, 2))
+        else:
+            layers += [nn.Conv2d(cin, v, 3, padding=1), nn.BatchNorm2d(v), nn.ReLU(inplace=True)]
+            cin = v
+    return tuple(_VGGSlice(*layers[a:b]) for a, b in VGG16_SLICES)
 
 
 class WSConv2d(nn.Conv2d):

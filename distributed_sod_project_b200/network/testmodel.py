@@ -3,7 +3,9 @@
 (`backbone.wsgn.from_wsgn.Backbone_ResNet50_in3`, the one-import swap in network/TestModel.py:11), and
 `wsgn_resnext50` / `cp_wsgn_resnext50`: the same on its weight-standardised GroupNorm ResNeXt-50 32×4d
 (`Backbone_ResNeXt50_in3`, built as `l_resnext50(pretrained, baseWidth=4, cardinality=32)`: the reference's builder
-omits those two arguments, and its X-50-GN-WS release is 32×4d).
+omits those two arguments, and its X-50-GN-WS release is 32×4d), and
+`vgg16` / `cp_vgg16`: the same decoder on the reference's VGG16-BN (`backbone.origin.from_origin.Backbone_VGG16_in3`), whose
+five slices carry 64 … 512 channels at strides 1 … 16.
 
 Zero-arg factories looked up by name from `user_config["model"]` (reference train.py:141):
 ResNet-50 encoder → five 1×1 "trans" convs to 64 ch → top-down decoder of SIM + ConvBNReLU with
@@ -19,7 +21,8 @@ import torch
 import torch.nn as nn
 from torch.utils.checkpoint import checkpoint
 
-from .blocks import SIM, ConvBNReLU, WSConv2d, bilinear, group_norm32, resnet50_stages, upsample_add
+from .blocks import (SIM, VGG16_SLICES, ConvBNReLU, WSConv2d, bilinear, group_norm32, resnet50_stages, upsample_add,
+                     vgg16_bn_slices)
 
 _TAPS = (32, 16, 8, 4, 2)                       # encoder strides tapped, deepest first
 _TAP_CHANNELS = {32: 2048, 16: 1024, 8: 512, 4: 256, 2: 64}
@@ -28,12 +31,13 @@ _TAP_CHANNELS = {32: 2048, 16: 1024, 8: 512, 4: 256, 2: 64}
 class _TestModel(nn.Module):
     recompute = False  # cp_res50 flips this
     backbone = staticmethod(resnet50_stages)
+    tap_channels = _TAP_CHANNELS                # channels of each backbone slice, keyed by its position name
 
     def __init__(self):
         super().__init__()
         self.div_2, self.div_4, self.div_8, self.div_16, self.div_32 = self.backbone()
         for s in _TAPS:
-            setattr(self, f"trans{s}", nn.Conv2d(_TAP_CHANNELS[s], 64, 1, 1))
+            setattr(self, f"trans{s}", nn.Conv2d(self.tap_channels[s], 64, 1, 1))
         for s in _TAPS:
             setattr(self, f"sim{s}", SIM(64, 32))
         for s in _TAPS:
@@ -119,27 +123,67 @@ class cp_wsgn_resnext50(wsgn_resnext50):
     recompute = True
 
 
+class vgg16(_TestModel):
+    """Plain variant on VGG16-BN (reference backbone/origin/from_origin.py:18-25).  `div_2` … `div_32` name slice
+    positions; their strides are 1, 2, 4, 8 and 16.  `div_2` is already at full resolution, so the head has no ×2
+    up-sample."""
+
+    backbone = staticmethod(vgg16_bn_slices)
+    tap_channels = {32: 512, 16: 512, 8: 256, 4: 128, 2: 64}
+
+    def _head(self, d2):
+        return self.classifier(self.upconv1(d2))
+
+
+class cp_vgg16(vgg16):
+    """Activation-checkpointed twin of `vgg16`, with the same twelve segments as `cp_res50`."""
+
+    recompute = True
+
+
+_RESNET_REMAP = {"conv1.": "div_2.0.", "bn1.": "div_2.1.", "layer1.": "div_4.1.", "layer2.": "div_8.",
+                 "layer3.": "div_16.", "layer4.": "div_32."}
+
+
+def _resnet_remap(k: str) -> str | None:
+    """torchvision / WS-GN ResNet key → `div_*` key by its first matching prefix, else None"""
+    for old, new in _RESNET_REMAP.items():
+        if k.startswith(old):
+            return new + k[len(old):]
+    return None
+
+
+def _vgg_remap(k: str) -> str | None:
+    """torchvision `vgg16_bn` key `features.{i}.*` → `div_*.{i - a}.*` of the slice that holds features[i], else None"""
+    if not k.startswith("features."):
+        return None
+    idx, _, rest = k[len("features."):].partition(".")
+    if not idx.isdigit():
+        return None
+    for name, (a, b) in zip(("div_2", "div_4", "div_8", "div_16", "div_32"), VGG16_SLICES):
+        if a <= int(idx) < b:
+            return f"{name}.{int(idx) - a}.{rest}"
+    return None
+
+
 def load_pretrained_backbone(model: _TestModel, path: str) -> list[str]:
     """Load ResNet-50 weights from a local file into `div_*` (the reference downloads them,
     backbone/origin/resnet.py:199-217 and backbone/wsgn/customized_func.py:32-43; no network here): torchvision's
     format, or the WS-GN release's — tensors under "state_dict", keys prefixed `module.` (stripped as the reference's
     `load_pretrained_params` does).  Keeps the reference's filter-then-update semantics: unknown keys are ignored.
-    Returns loaded keys."""
+    For `vgg16` / `cp_vgg16` it reads torchvision's `vgg16_bn` file: `features.{i}.*` goes to the slice holding
+    features[i], `classifier.*` is ignored.  Returns loaded keys."""
     src = torch.load(path, map_location="cpu")
     if isinstance(src.get("state_dict"), dict):
         src = src["state_dict"]
     src = {k[len("module."):] if k.startswith("module.") else k: v for k, v in src.items()}
-    remap = {"conv1.": "div_2.0.", "bn1.": "div_2.1.", "layer1.": "div_4.1.", "layer2.": "div_8.",
-             "layer3.": "div_16.", "layer4.": "div_32."}
+    rename = _vgg_remap if isinstance(model, vgg16) else _resnet_remap
     own = model.state_dict()
     picked = {}
     for k, v in src.items():
-        for old, new in remap.items():
-            if k.startswith(old):
-                nk = new + k[len(old):]
-                if nk in own and own[nk].shape == v.shape:
-                    picked[nk] = v
-                break
+        nk = rename(k)
+        if nk in own and own[nk].shape == v.shape:
+            picked[nk] = v
     own.update(picked)
     model.load_state_dict(own)
     return sorted(picked)

@@ -14,7 +14,8 @@ import torch
 from . import _lib
 
 ENABLED = False     # switched on by the engine (engine.Trainer)
-# the stem's MaxPool2d(3, 2, 1) through csrc/maxpool.cu (checked against torch by tests/test_gpu_resample.py; SOD_MAXPOOL=0 → torch op)
+# the ResNet stem's MaxPool2d(3, 2, 1) and VGG16-BN's MaxPool2d(2, 2) through csrc/maxpool.cu (checked against torch by
+# tests/test_gpu_resample.py and tests/test_gpu_maxpool2.py; SOD_MAXPOOL=0 → torch op)
 MAXPOOL_ENABLED = os.environ.get("SOD_MAXPOOL", "1") == "1"
 # bias gradient of the convolutions that do not feed a BatchNorm as a deterministic column sum (SOD_COLSUM=0 → autograd's reduction)
 COLSUM_ENABLED = os.environ.get("SOD_COLSUM", "1") == "1"
@@ -135,6 +136,42 @@ def maxpool3x3s2(x: torch.Tensor) -> torch.Tensor | None:
     if not (MAXPOOL_ENABLED and _ok(x)):
         return None
     return _MaxPool3x3s2.apply(x)
+
+
+class _MaxPool2x2s2(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x):
+        x = _rows(x)
+        n, c, h, w = x.shape
+        y = torch.empty((n, c, h // 2, w // 2), dtype=x.dtype, device=x.device, memory_format=torch.channels_last)
+        arg = torch.empty(y.numel(), dtype=torch.uint8, device=x.device)      # window position kh*2+kw per element
+        rc = _lib.lib().sod_maxpool2x2s2_fwd(x.data_ptr(), y.data_ptr(), arg.data_ptr(), n, h, w, c, _lib.dtype_code(x.dtype),
+                                             _lib.stream_ptr())
+        _lib.check(rc, "sod_maxpool2x2s2_fwd")
+        _lib.count_launch()
+        ctx.shape = (n, c, h, w)
+        ctx.save_for_backward(arg)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        (arg,) = ctx.saved_tensors
+        n, c, h, w = ctx.shape
+        dy = _rows(dy)
+        dx = torch.empty((n, c, h, w), dtype=dy.dtype, device=dy.device, memory_format=torch.channels_last)
+        rc = _lib.lib().sod_maxpool2x2s2_bwd(dy.data_ptr(), arg.data_ptr(), dx.data_ptr(), n, h, w, c, _lib.dtype_code(dy.dtype),
+                                             _lib.stream_ptr())
+        _lib.check(rc, "sod_maxpool2x2s2_bwd")
+        _lib.count_launch()
+        return dx
+
+
+def maxpool2x2s2(x: torch.Tensor) -> torch.Tensor | None:
+    """MaxPool2d(2, stride 2) of VGG16-BN, floor mode; None (caller keeps the torch op) when the kernel is switched off or
+    does not cover x"""
+    if not (MAXPOOL_ENABLED and _ok(x)) or x.shape[2] < 2 or x.shape[3] < 2:
+        return None
+    return _MaxPool2x2s2.apply(x)
 
 
 # ---- convolution whose bias gradient is a deterministic column sum (csrc/resample.cu: sod_colsum) ------------------------

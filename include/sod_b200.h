@@ -382,6 +382,16 @@ int sod_gconv3x3_wgrad(const void* x, const void* dy, float* dw_hat, int dtype, 
 int sod_maxpool3x3s2_fwd(const void* x, void* y, void* argmax, int n, int h, int w, int c, int dtype, void* stream);
 int sod_maxpool3x3s2_bwd(const void* dy, const void* argmax, void* dx, int n, int h, int w, int c, int dtype, void* stream);
 
+/* MaxPool2d(kernel 2, stride 2) of VGG16-BN (backbone/origin/vgg.py `make_layers` "M"; the first op of `div_4` … `div_32`
+ * in backbone/origin/from_origin.py:18-25), channels-last [N,H,W,C], fp32 / bf16 / fp16; (h, w) = INPUT size, output
+ * (h/2, w/2) (floor mode).  argmax: one byte per OUTPUT element (window position kh*2+kw, or 4 for a window with
+ * nothing above -inf other than the first, where torch's index points outside the window).  Ties / NaN as torch: first
+ * maximum in (kh, kw) scan order, NaN propagates.  The backward writes every dx element: dy at the window position the
+ * byte names, 0 elsewhere and on the row / column floor mode drops (bit-identical to torch's).  h < 2, w < 2 or
+ * C % 8 != 0 → SOD_EUNSUPPORTED, a pointer not 16-byte aligned → SOD_EALIGN; a refused call writes nothing. */
+int sod_maxpool2x2s2_fwd(const void* x, void* y, void* argmax, int n, int h, int w, int c, int dtype, void* stream);
+int sod_maxpool2x2s2_bwd(const void* dy, const void* argmax, void* dx, int n, int h, int w, int c, int dtype, void* stream);
+
 /* ------------------------------------------------------------------------------------------------
  * Data-side neighbours of the iteration (SURVEY §8f.2, §8f.4).
  *
