@@ -4,12 +4,9 @@ import numpy as np
 import pytest
 import torch
 
+from _backbones import _trainer
+
 pytestmark = pytest.mark.gpu
-
-
-def _trainer(model_name, **kw):
-    from distributed_sod_project_b200.engine import Trainer
-    return Trainer(model_name=model_name, lr=0.05, momentum=0.9, weight_decay=5e-4, **kw)
 
 
 @pytest.mark.parametrize("tag,model", [("res50_w1_s128", "res50"), ("res50_w1_s64", "res50"), ("cp_res50_w1_s64", "cp_res50")])

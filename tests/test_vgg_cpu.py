@@ -1,12 +1,10 @@
-"""CPU checks of the VGG16-BN plugins (`vgg16`, `cp_vgg16`): bit-identity with the reference's TestModel composed on
-`Backbone_VGG16_in3`, names, counts and optimizer groups, torchvision's `vgg16_bn` file format, the CPU routing of the
-2×2 pools, and the C ABI of the 2×2 max-pool entries."""
+"""CPU checks of the VGG16-BN plugins (`vgg16`, `cp_vgg16`): names and counts, torchvision's `vgg16_bn` file format,
+the CPU routing of the 2×2 pools, and the C ABI of the 2×2 max-pool entries.  Bit-identity with the reference and the
+f3_trick groups are checked for every backbone in tests/test_backbones_cpu.py."""
 from __future__ import annotations
 
 import os
 
-import numpy as np
-import pytest
 import torch
 import torch.nn as nn
 import torch.nn.functional as F
@@ -21,35 +19,8 @@ def _model(name="vgg16"):
     return getattr(network, name)()
 
 
-@pytest.mark.parametrize("name", ["vgg16", "cp_vgg16"])
-def test_plugin_is_bit_identical_to_reference(golden, name):
-    """init_seed(0) + the plugin against the reference composition (tests/golden/model_vgg16_init.npz,
-    tools/make_golden_vgg.py): keys in order, shapes, values at fixed positions, per-tensor sums and one training-mode
-    forward at 8 threads.  The first convolution's biases are torch's default uniform init, not zero"""
-    g = golden("model_vgg16_init.npz")
-    m = _model(name)
-    sd = m.state_dict()
-    assert "\n".join(sd) == str(g["keys"])
-    for i, v in enumerate(sd.values()):
-        assert list(v.shape) == [d for d in g["shapes"][i] if d >= 0]
-        a = v.detach().reshape(-1).double()
-        idx = torch.from_numpy(np.linspace(0, a.numel() - 1, g["values"].shape[1]).astype(np.int64))
-        np.testing.assert_array_equal(a[idx].numpy(), g["values"][i])
-        np.testing.assert_allclose([a.sum().item(), (a * a).sum().item()], g["moments"][i], rtol=1e-12, atol=0)
-    assert 0.05 < float(m.div_2[0].bias.detach().abs().mean()) < 0.15
-    threads = torch.get_num_threads()
-    torch.set_num_threads(8)
-    try:
-        y = m(torch.from_numpy(g["x"])).detach().numpy()
-    finally:
-        torch.set_num_threads(threads)
-    assert y.shape == g["x"].shape[:1] + (1,) + g["x"].shape[2:]          # full resolution: no ×2 head up-sample
-    np.testing.assert_array_equal(y, g["y"])
-
-
-def test_names_counts_and_f3_trick_groups():
+def test_names_and_counts():
     from distributed_sod_project_b200.network.blocks import _VGGPool
-    from distributed_sod_project_b200.optim import make_optimizer
     m = _model()
     backbone = [m.div_2, m.div_4, m.div_8, m.div_16, m.div_32]
     assert [len(s) for s in backbone] == [6, 7, 10, 10, 10]
@@ -64,12 +35,8 @@ def test_names_counts_and_f3_trick_groups():
     assert sum(p.numel() for n, p in m.named_parameters() if n.startswith("div")) == 14_723_136
     sd = m.state_dict()
     assert "div_4.1.weight" in sd and "div_4.2.running_var" in sd and "div_32.8.bias" in sd and "div_32.10.weight" not in sd
-    opt = make_optimizer(m, "f3_trick", dict(lr=0.05, momentum=0.9, weight_decay=5e-4, nesterov=False))
-    names = [n for n, _ in m.named_parameters()]
-    groups = [[n for n, p in m.named_parameters() if any(p is q for q in g["params"])] for g in opt.param_groups]
-    assert all(n.startswith("div") and not n.startswith("div_2") for n in groups[0])
-    assert all(not n.startswith("div") for n in groups[1])
-    assert set(names) - set(groups[0]) - set(groups[1]) == {f"div_2.{i}.{k}" for i in (0, 1, 3, 4) for k in ("weight", "bias")}
+    # the reference keeps torch's default init: the first convolution's biases are uniform, not zero
+    assert 0.05 < float(m.div_2[0].bias.detach().abs().mean()) < 0.15
 
 
 def test_cpu_forward_keeps_the_torch_pool():

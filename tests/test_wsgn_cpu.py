@@ -1,6 +1,7 @@
-"""CPU checks of the WS-GN plugins (`wsgn_res50`, `cp_wsgn_res50`): bit-identity with the reference's weight-standardised
-GroupNorm ResNet-50 TestModel, names and optimizer groups, the WS-GN release's pretrained file format, the fp64 oracle
-of csrc/wsgn.cu, its launch-geometry model and the C ABI of the new entries."""
+"""CPU checks of the WS-GN plugins (`wsgn_res50`, `cp_wsgn_res50`): names, norms and the WS convolutions' fp32 ranges,
+the WS-GN release's pretrained file format, the fp64 oracle of csrc/wsgn.cu, its launch-geometry model and the C ABI of
+the new entries.  Bit-identity with the reference and the f3_trick groups are checked for every backbone in
+tests/test_backbones_cpu.py."""
 from __future__ import annotations
 
 import ctypes
@@ -24,31 +25,7 @@ def _model(name="wsgn_res50"):
     return getattr(network, name)()
 
 
-@pytest.mark.parametrize("name", ["wsgn_res50", "cp_wsgn_res50"])
-def test_wsgn_plugin_is_bit_identical_to_reference(golden, name):
-    """init_seed(0) + the plugin against the reference TestModel on backbone.wsgn (tests/golden/model_wsgn_res50_init.npz,
-    tools/make_golden_wsgn.py): same keys and shapes, the same values at fixed positions and per-tensor sums, and the
-    same output of one training-mode forward at the 8 threads the vectors were made with"""
-    g = golden("model_wsgn_res50_init.npz")
-    m = _model(name)
-    sd = m.state_dict()
-    assert "\n".join(sd) == str(g["keys"])
-    for i, v in enumerate(sd.values()):
-        assert list(v.shape) == [d for d in g["shapes"][i] if d >= 0]
-        a = v.detach().reshape(-1).double()
-        idx = torch.from_numpy(np.linspace(0, a.numel() - 1, g["values"].shape[1]).astype(np.int64))
-        np.testing.assert_array_equal(a[idx].numpy(), g["values"][i])
-        np.testing.assert_allclose([a.sum().item(), (a * a).sum().item()], g["moments"][i], rtol=1e-12, atol=0)
-    threads = torch.get_num_threads()
-    torch.set_num_threads(8)
-    try:
-        y = m(torch.from_numpy(g["x"])).detach().numpy()
-    finally:
-        torch.set_num_threads(threads)
-    np.testing.assert_array_equal(y, g["y"])
-
-
-def test_wsgn_names_norms_and_f3_trick_groups():
+def test_wsgn_names_norms_and_ws_ranges():
     from distributed_sod_project_b200.network.blocks import WSConv2d
     from distributed_sod_project_b200.optim import make_optimizer
     m = _model()
@@ -61,12 +38,6 @@ def test_wsgn_names_norms_and_f3_trick_groups():
     assert all(not b.startswith("div") for b, _ in m.named_buffers())
     assert sum(isinstance(x, nn.BatchNorm2d) for x in m.modules()) == 84 - 53
     opt = make_optimizer(m, "f3_trick", dict(lr=0.05, momentum=0.9, weight_decay=5e-4, nesterov=False))
-    grouped = [[n for n, p in m.named_parameters() if any(p is q for q in g["params"])] for g in opt.param_groups]
-    assert [g["lr"] for g in opt.param_groups] == pytest.approx([0.005, 0.05])
-    assert all(n.startswith("div") and not n.startswith("div_2") for n in grouped[0])
-    assert all(not n.startswith("div") for n in grouped[1])
-    frozen = set(names) - set(grouped[0]) - set(grouped[1])
-    assert frozen == {"div_2.0.weight", "div_2.1.weight", "div_2.1.bias"}
     # no WS convolution's parameters are in the optimizer's 16-bit gradient part of the flat buffer
     ws_ids = {id(x.weight) for x in m.modules() if isinstance(x, WSConv2d)}
     f = opt.flat

@@ -193,7 +193,7 @@ def step_vectors(model_name: str, world: int, bs: int, size: int, iters: int, ta
 def model_init_vectors(model_name: str = "res50", samples: int = 32, tag: str | None = None):
     """the reference model right after `init_seed(0)`: every state_dict key and shape, per-tensor float64 sum and sum of
     squares, a fixed seeded sample of values per tensor, and the output of one forward pass on a seeded input
-    (tests/test_host_cpu.py::test_model_plugin_is_bit_identical_to_reference compares the package's plugin with it)"""
+    (tests/test_backbones_cpu.py::test_model_plugin_is_bit_identical_to_reference compares the package's plugin with it)"""
     import network
     from utils.misc import init_seed
     init_seed(0)
