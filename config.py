@@ -9,6 +9,16 @@ Extra keys (all optional, defaults reproduce the benchmark configuration):
   channels_last   run the network in NHWC (what cuDNN's tensor-core kernels and the SyncBN kernels want)
   synthetic       train on synthetic batches of the dataloader's output contract; False: train on
                   `rgb_data.tr_data_path` with the reference's resize and augmentation run on the GPU (train.py)
+  joint_transforms  with `synthetic` False: the reference's joint transforms (utils/joint_transforms.py) to train with,
+                  a list of [name, *args] entries in application order, with the reference's constructor arguments:
+                  ["JointResize", size], ["ScaleCenterCrop", input_size], ["PaddingSquare", pad_size],
+                  ["RandomScaleCrop", input_size, scale_factor], ["RandomHorizontallyFlip"], ["RandomRotate", degree],
+                  ["RandomGaussianBlur"].  Accepted order: exactly one size step first (JointResize, ScaleCenterCrop
+                  or PaddingSquare), then optionally RandomScaleCrop (its input_size is the size step's side), then
+                  RandomHorizontallyFlip, RandomRotate and RandomGaussianBlur, each optional, in that order; the chain
+                  must make `input_size`² samples.  Anything else is a ValueError naming the entry.  ColorJitter(0.1,
+                  0.1, 0.1) always follows.  Absent or None: the reference's [["JointResize", input_size],
+                  ["RandomHorizontallyFlip"], ["RandomRotate", 10]].  Evaluation is not affected.
   cuda_graph      capture one iteration per (shape, lr) and replay it: one launch instead of ~700 kernel launches
   synthetic_eval  evaluate on synthetic sets of `synthetic_eval_images` images named after the configured sets; False:
                   read `te_data_list` / `val_data_path` from disk (a missing path is an error naming the set) and report

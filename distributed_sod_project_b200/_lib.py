@@ -77,6 +77,10 @@ class sod_augment_param(C.Structure):
                 ("factor", C.c_float * 3)]
 
 
+class sod_blur_param(C.Structure):
+    _fields_ = [("radius", C.c_int32), ("ww", C.c_uint32), ("fw", C.c_uint32)]
+
+
 _PROTOTYPES = {
     "sod_version": (C.c_int, []),
     "sod_strerror": (C.c_char_p, [C.c_int]),
@@ -158,7 +162,16 @@ _PROTOTYPES = {
     "sod_augment_u8_workspace_bytes": (C.c_size_t, [C.c_int]),
     "sod_augment_u8": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.POINTER(sod_augment_param),
                                  C.c_void_p, C.c_size_t, C.c_void_p]),
-    "sod_groupnorm_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int64, C.c_int, C.c_int]),
+    "sod_resize_nearest_u8_workspace_bytes": (C.c_size_t, [C.c_int, C.c_void_p, C.c_void_p, C.c_int]),
+    "sod_resize_nearest_u8": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                        C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "sod_window_u8_workspace_bytes": (C.c_size_t, [C.c_int]),
+    "sod_window_u8": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                C.c_int, C.c_int, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "sod_gaussian_blur_u8_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int, C.c_int]),
+    "sod_gaussian_blur_u8": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(sod_blur_param),
+                                       C.c_void_p, C.c_size_t, C.c_void_p]),
+    "sod_groupnorm_workspace_bytes":(C.c_size_t, [C.c_int, C.c_int64, C.c_int, C.c_int]),
     "sod_groupnorm_splits": (C.c_int, [C.c_int, C.c_int64, C.c_int, C.c_int]),
     "sod_groupnorm_fwd": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
                                     C.c_int64, C.c_int, C.c_int, C.c_float, C.c_int, C.c_void_p, C.c_size_t, C.c_void_p]),

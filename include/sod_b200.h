@@ -483,6 +483,46 @@ size_t sod_augment_u8_workspace_bytes(int n);
 int sod_augment_u8(const void* img, const void* mask, void* img_out, void* mask_out, int n, int size,
                    const sod_augment_param* params, void* workspace, size_t workspace_bytes, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * The reference's other joint transforms (utils/joint_transforms.py:51-137: RandomScaleCrop, ScaleCenterCrop,
+ * PaddingSquare, RandomGaussianBlur) are composed from sod_resize_u8, sod_augment_u8 and the three entries below, each
+ * bit for bit as Pillow computes it.  Ragged batches are laid out as for sod_resize_u8 (device offsets and sizes);
+ * the *_hw_host arrays are HOST copies of the same sizes, and every per-image parameter array is a HOST array that is
+ * copied into the workspace before the call returns.  Each *_workspace_bytes returns 0 for invalid arguments, and each
+ * entry returns SOD_EINVAL on a null pointer, n <= 0, channels other than 1 ("L") or 3 ("RGB", HWC), a non-positive
+ * size or a workspace smaller than its query.  src and dst must not overlap.
+ *
+ * sod_resize_nearest_u8 — `Image.resize((w, h), NEAREST)`: per axis a = in / out and the source index of output pixel
+ * x is (int)xo with xo = a·0.5, then xo += a per pixel, accumulated in double as Pillow does.  Two launches.
+ * ------------------------------------------------------------------------------------------------ */
+size_t sod_resize_nearest_u8_workspace_bytes(int n, const int32_t* src_hw, const int32_t* dst_hw, int channels);
+int sod_resize_nearest_u8(const void* src, const int64_t* src_off, const int32_t* src_hw, void* dst, const int64_t* dst_off,
+                          const int32_t* dst_hw, const int32_t* src_hw_host, const int32_t* dst_hw_host, int n, int channels,
+                          void* workspace, size_t workspace_bytes, void* stream);
+
+/* sod_window_u8 — image i of dst (dst_hw[i]) is the window of image i of src at offset[2i] rows, offset[2i+1] columns
+ * (either may be negative), 0 outside the source: `Image.crop` for RandomScaleCrop / ScaleCenterCrop, and the centred
+ * zero padding of PaddingSquare.  One launch. */
+size_t sod_window_u8_workspace_bytes(int n);
+int sod_window_u8(const void* src, const int64_t* src_off, const int32_t* src_hw, void* dst, const int64_t* dst_off,
+                  const int32_t* dst_hw, const int32_t* dst_hw_host, const int32_t* offset, int n, int channels,
+                  void* workspace, size_t workspace_bytes, void* stream);
+
+/* sod_gaussian_blur_u8 — `img.filter(ImageFilter.GaussianBlur(r))` on n equal-size h × w images, one r per image given
+ * as Pillow's box parameters (libImaging/BoxBlur.c): radius = (int)rad, ww = (uint32)(2^24 / (2·rad + 1)) in float32,
+ * fw = (2^24 − (2·radius + 1)·ww) / 2, with rad Pillow's extended-box radius of r for three passes.  Three horizontal
+ * passes, then three vertical, each (ww·Σ_{|k|≤radius} x[i+k] + fw·(x[i−radius−1] + x[i+radius+1]) + 2^23) >> 24 with
+ * edge clamping.  radius 0 with ww = 2^24, fw = 0 is the identity (Pillow's copy at r = 0).  A parameter with radius
+ * outside [0, 1024], ww = 0 or (2·radius + 1)·ww + 2·fw > 2^24 is SOD_EINVAL.  Six launches. */
+typedef struct sod_blur_param {
+    int32_t radius;
+    uint32_t ww;
+    uint32_t fw;
+} sod_blur_param;
+size_t sod_gaussian_blur_u8_workspace_bytes(int n, int h, int w, int channels);
+int sod_gaussian_blur_u8(const void* src, void* dst, int n, int h, int w, int channels, const sod_blur_param* params,
+                         void* workspace, size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -2,6 +2,7 @@
 """What training from an on-disk set costs.  Prints one JSON line.
 
     python tools/bench_train_disk.py [--images 512] [--batch 16] [--size 320] [--workers 4 8] [--iters 200]
+                                     [--joint-transforms '[["JointResize", 320], ["RandomScaleCrop", 320, 1.5], ...]']
 
 In one run, on the current GPU (its name and power limit are part of the output):
 * writes a seeded training set under a temporary directory: `--images` JPEG images of 300–500 px in both orientations,
@@ -15,6 +16,11 @@ In one run, on the current GPU (its name and power limit are part of the output)
 * `train_img_s`: end-to-end training images/s from disk (res50, bf16, CUDA-graph replay, the benchmark's
   configuration), per worker count, over one whole epoch after a warm-up epoch;
 * `synthetic_device_img_s`: the same trainer on a device-resident batch, i.e. the iteration alone.
+With `--joint-transforms` (a `joint_transforms` list as config.py takes it), also:
+* `joint_gpu_us_per_batch`: the chain's stages on the same batch after warm-up: the size step, RandomScaleCrop, the
+  blur (on the drawn radii: about half the samples blur, the others run the identity box), the whole chain with
+  ColorJitter (`joint_chain_u8`), and the chain plus `preprocess_batch`;
+* `joint_train_img_s`: end-to-end training images/s from disk with the chain, per worker count.
 """
 from __future__ import annotations
 
@@ -53,6 +59,8 @@ def main() -> None:
     ap.add_argument("--size", type=int, default=320)
     ap.add_argument("--workers", type=int, nargs="+", default=[4, 8])
     ap.add_argument("--iters", type=int, default=200)
+    ap.add_argument("--joint-transforms", type=json.loads, default=None,
+                    help="a joint_transforms chain (JSON) measured besides the reference's")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("bench_train_disk.py measures on a GPU")
@@ -63,7 +71,9 @@ def main() -> None:
     from distributed_sod_project_b200 import _lib
     from distributed_sod_project_b200.data import make_train_loader
     from distributed_sod_project_b200.engine import Trainer
-    from distributed_sod_project_b200.pipeline import (Ragged, TrainPrefetcher, augment_u8, draw_augment_params, preprocess_batch,
+    from distributed_sod_project_b200.pipeline import (Ragged, TrainPrefetcher, augment_u8, draw_augment_params,
+                                                       draw_joint_params, gaussian_blur_u8, joint_chain_u8, joint_size_step,
+                                                       parse_joint_transforms, preprocess_batch, random_scale_crop,
                                                        resize_u8)
 
     torch.cuda.set_device(0)
@@ -96,6 +106,21 @@ def main() -> None:
             "preprocess": round(_events_us(lambda: preprocess_batch(ai, am), args.iters), 1),
             "all": round(_events_us(chain, args.iters), 1),
         }
+
+        chain = parse_joint_transforms(args.joint_transforms, S) if args.joint_transforms is not None else None
+        if chain is not None:
+            result["joint_transforms"] = chain
+            jp = draw_joint_params(bs, chain, torch.Generator().manual_seed(0))
+            us = {"size_step": round(_events_us(lambda: joint_size_step(chain[0], img, mask), args.iters), 1)}
+            si, sm = joint_size_step(chain[0], img, mask)
+            if jp.crop is not None:
+                us["random_scale_crop"] = round(_events_us(lambda: random_scale_crop(si, sm, jp.crop), args.iters), 1)
+            if jp.blur is not None:
+                bi = si.as_batch().contiguous()
+                us["gaussian_blur"] = round(_events_us(lambda: gaussian_blur_u8(bi, jp.blur), args.iters), 1)
+            us["chain_with_jitter"] = round(_events_us(lambda: joint_chain_u8(chain, jp, img, mask), args.iters), 1)
+            us["all"] = round(_events_us(lambda: preprocess_batch(*joint_chain_u8(chain, jp, img, mask)), args.iters), 1)
+            result["joint_gpu_us_per_batch"] = us
 
         # the reference's host chain on the same batch, decoded images in hand
         norm = T.Normalize([0.485, 0.456, 0.406], [0.229, 0.224, 0.225])
@@ -134,6 +159,12 @@ def main() -> None:
             pf = TrainPrefetcher(make_train_loader(root, bs, num_workers=w), S, seed=0)
             _epoch_img_s(trainer, pf, 0)                                            # warm-up: graph capture, cuDNN
             result["train_img_s"][str(w)] = round(_epoch_img_s(trainer, pf, 1), 1)
+        if chain is not None:
+            result["joint_train_img_s"] = {}
+            for w in args.workers:
+                pf = TrainPrefetcher(make_train_loader(root, bs, num_workers=w), S, seed=0, joint_transforms=chain)
+                _epoch_img_s(trainer, pf, 0)
+                result["joint_train_img_s"][str(w)] = round(_epoch_img_s(trainer, pf, 1), 1)
         x, m, _ = next(iter(TrainPrefetcher(make_train_loader(root, bs, num_workers=0), S, seed=0)))
         steps = args.images // bs
         for _ in range(5):

@@ -122,7 +122,8 @@ def main_worker(local_rank, ngpus_per_node, world_size, args, exp_name, path_con
         rank, world = (dist.get_rank(), dist.get_world_size()) if dist.is_initialized() else (0, 1)
         source = make_train_loader(cfg["rgb_data"]["tr_data_path"], batch_size_single_gpu, world, rank, cfg["num_workers"],
                                    cfg["prefix"])
-        loader = TrainPrefetcher(source, cfg["input_size"], size_list=cfg["size_list"], seed=0, rank=rank)
+        loader = TrainPrefetcher(source, cfg["input_size"], size_list=cfg["size_list"], seed=0, rank=rank,
+                                 joint_transforms=cfg.get("joint_transforms"))
     elif cfg.get("synthetic_uint8", True):
         # SURVEY §8f.2: uint8 batches from the (here: synthetic) workers, pinned → H2D and ToTensor / Normalize / multi-scale
         # collate as one GPU kernel, one batch ahead of the iteration (reference: BackgroundGenerator, train.py:285)
