@@ -1,12 +1,21 @@
-"""Block "sites" of `res50`: the model cut into the pieces `_TestModel.forward` strings together, so that each can be run
-and differentiated on its own (tests/test_block_sites_cpu.py, tests/test_gpu_block_seams.py).
+"""Block "sites" of the four TestModel backbones (`res50`, `vgg16`, `wsgn_res50`, `wsgn_resnext50`): each model cut into
+the pieces `_TestModel.forward` strings together, so that each can be run and differentiated on its own
+(tests/test_block_sites_cpu.py, tests/test_gpu_block_seams.py).  Every function takes the model's name, `res50` by
+default.
 
 A site owns the parameters and buffers under its module paths (every one of the model's belongs to exactly one site),
 takes its inputs at image size S from `shapes(S, batch)` and runs as `run(mods, *inputs)`, `mods` mapping each path to a
-module — the engine's own, or the float64 copies `stock_twin` makes.  `dispatch(site, S, amp)` says which backward nodes
-of the engine's autograd seam (`_SyncBNFnBackward`, `_Up2xBackward`, …) its forward must create: that follows the
-predicates of `resample.py` (C % 8 == 0; ×2 exactly; even H and W for the 2×2 pool; `conv_bias`: C a power of two times
-8, only reached by the `trans*` convolutions under amp shadow weights) at the shapes the site sees.
+module — the engine's own, or the float64 copies `stock_twin` makes.  `dispatch(site, S, amp, model_name)` says which
+backward nodes of the engine's autograd seam (`_SyncBNFnBackward`, `_Up2xBackward`, `_GroupNormFnBackward`, …) its
+forward must create: that follows the predicates of `resample.py` (C % 8 == 0; ×2 exactly; even H and W for the 2×2
+average pool; `conv_bias`: C a power of two times 8, only reached by the `trans*` convolutions under amp shadow weights)
+and of `wsgn.py` (the grouped-convolution kernels run only where `grouped_conv_on_kernels` holds) at the shapes the site
+sees.
+
+* `wsgn_res50` / `wsgn_resnext50` have `res50`'s sites (paths, shapes, representatives); their backbone norms are
+  GroupNorm(32) and their convolutions weight-standardised, their decoder is `res50`'s.
+* `vgg16`'s backbone sites are its five slices `div_2` … `div_32`, at strides 1 … 16; `div_4` … `div_32` open with a 2×2
+  max-pool.  Its decoder sites carry `res50`'s names at half `res50`'s stride, and its head has no ×2 up-sample.
 """
 from __future__ import annotations
 
@@ -21,21 +30,26 @@ TAPS = (32, 16, 8, 4, 2)
 TAP_CHANNELS = {32: 2048, 16: 1024, 8: 512, 4: 256, 2: 64}
 STAGES = ((4, 64, 3), (8, 128, 4), (16, 256, 6), (32, 512, 3))     # (stride, width, units) of ResNet-50
 SIZES = (256, 288, 320, 352, 384)                                  # 288 / 352: odd 9×9 / 11×11 stride-32 map
+MODELS = ("res50", "vgg16", "wsgn_res50", "wsgn_resnext50")
+WSGN = ("wsgn_res50", "wsgn_resnext50")
+VGG_TAP_CHANNELS = {32: 512, 16: 512, 8: 256, 4: 128, 2: 64}       # `vgg16.tap_channels`
+VGG_SLICE_IN = {2: 3, 4: 64, 8: 128, 16: 256, 32: 512}             # input channels of slice div_s, at stride s // 4 (div_2: 1)
 
 BN, UP, AVG, MAX, CONVB, LOSS = ("_SyncBNFnBackward", "_Up2xBackward", "_AvgPool2x2Backward", "_MaxPool3x3s2Backward",
                                  "_ConvBiasBackward", "_FusedLossFnBackward")
-SEAM_NODES = (BN, UP, AVG, MAX, CONVB)
+GN, WS, WSG, MAX2 = "_GroupNormFnBackward", "_WSFnBackward", "_WSGroupConvFnBackward", "_MaxPool2x2s2Backward"
+SEAM_NODES = (BN, UP, AVG, MAX, CONVB, GN, WS, WSG, MAX2)
 
 
 @dataclass(frozen=True)
 class Site:
     name: str
-    paths: tuple[str, ...]                    # module paths of res50 whose parameters / buffers the site owns
+    paths: tuple[str, ...]                    # module paths of the model whose parameters / buffers the site owns
     shapes: Callable[[int, int], list]        # (S, batch) → input shapes
     run: Callable                             # run(mods, *inputs) → output
-    kind: str                                 # stem | pool | down | plain | trans | sim | upconv | upadd | head
+    kind: str                                 # stem | pool | down | plain | vpool | trans | sim | upconv | upadd | head
     stride: int                               # stride of the site's input
-    representative: bool = True               # in the GPU grid (the other plain bottlenecks repeat a tested one)
+    representative: bool = True               # GPU grid (`grid`); the other plain bottlenecks repeat a tested one
     loss: bool = False                        # head: the fused BCE + CEL loss follows
     input_grad: tuple[bool, ...] = field(default=(True,))
 
@@ -64,7 +78,16 @@ def _head_run(mods, d2):
     return mods["classifier"](mods["upconv1"](bilinear(d2, scale_factor=2)))
 
 
-def sites() -> list[Site]:
+def _vgg_head_run(mods, d2):
+    return mods["classifier"](mods["upconv1"](d2))       # `vgg16._head`: d2 is already at full resolution
+
+
+def _check(model_name):
+    if model_name not in MODELS:
+        raise ValueError(f"no site table for model {model_name!r}; one of {MODELS}")
+
+
+def _resnet_backbone() -> list[Site]:
     out = [Site("stem", ("div_2",), lambda S, b: [(b, 3, S, S)], lambda mods, x: mods["div_2"](x), "stem", 1),
            Site("pool+div_4.1.0", ("div_4.0", "div_4.1.0"), lambda S, b: [(b, 64, S // 2, S // 2)],
                 lambda mods, x: mods["div_4.1.0"](mods["div_4.0"](x)), "pool", 2)]
@@ -74,62 +97,114 @@ def sites() -> list[Site]:
             if not (stride == 4 and u == 0):
                 out.append(_bottleneck_site(stride, u, cin, width, down=u == 0))
             cin = 4 * width
-    for s in TAPS:
-        out.append(Site(f"trans{s}", (f"trans{s}",), lambda S, b, s=s: [(b, TAP_CHANNELS[s], S // s, S // s)],
-                        lambda mods, x, s=s: mods[f"trans{s}"](x), "trans", s))
-    for s in TAPS:
-        out.append(Site(f"sim{s}", (f"sim{s}",), lambda S, b, s=s: [(b, 64, S // s, S // s)], _sim_run(s), "sim", s))
-    for s in TAPS:
-        out.append(Site(f"upconv{s}", (f"upconv{s}",), lambda S, b, s=s: [(b, 64, S // s, S // s)],
-                        lambda mods, x, s=s: mods[f"upconv{s}"](x), "upconv", s))
-    for s in TAPS[1:]:
-        out.append(Site(f"upsample_add{s}", (), lambda S, b, s=s: [(b, 64, S // (2 * s), S // (2 * s)), (b, 64, S // s, S // s)],
-                        _upadd_run, "upadd", s, input_grad=(True, True)))
-    out.append(Site("head", ("upconv1", "classifier"), lambda S, b: [(b, 32, S // 2, S // 2)], _head_run, "head", 2,
-                    loss=True))
     return out
 
 
-def by_name() -> dict[str, Site]:
-    return {s.name: s for s in sites()}
+def _vgg_backbone() -> list[Site]:
+    out = []
+    for s in reversed(TAPS):
+        st = max(s // 4, 1)                  # div_2 and div_4 both see the full-resolution map
+        out.append(Site(f"div_{s}", (f"div_{s}",), lambda S, b, c=VGG_SLICE_IN[s], st=st: [(b, c, S // st, S // st)],
+                        lambda mods, x, s=s: mods[f"div_{s}"](x), "stem" if s == 2 else "vpool", st))
+    return out
+
+
+def _decoder(tap_channels, half) -> list[Site]:
+    """trans* … head; `half`: every tap sits at half `res50`'s stride (vgg16)"""
+    st = {s: s // 2 if half else s for s in TAPS}
+    out = []
+    for s in TAPS:
+        out.append(Site(f"trans{s}", (f"trans{s}",), lambda S, b, s=s: [(b, tap_channels[s], S // st[s], S // st[s])],
+                        lambda mods, x, s=s: mods[f"trans{s}"](x), "trans", st[s]))
+    for s in TAPS:
+        out.append(Site(f"sim{s}", (f"sim{s}",), lambda S, b, s=s: [(b, 64, S // st[s], S // st[s])], _sim_run(s), "sim",
+                        st[s]))
+    for s in TAPS:
+        out.append(Site(f"upconv{s}", (f"upconv{s}",), lambda S, b, s=s: [(b, 64, S // st[s], S // st[s])],
+                        lambda mods, x, s=s: mods[f"upconv{s}"](x), "upconv", st[s]))
+    for s in TAPS[1:]:
+        out.append(Site(f"upsample_add{s}", (), lambda S, b, s=s: [(b, 64, S // (2 * st[s]), S // (2 * st[s])),
+                                                                   (b, 64, S // st[s], S // st[s])],
+                        _upadd_run, "upadd", st[s], input_grad=(True, True)))
+    h = st[2]                                # the head's input d2: up-sampled ×2 inside (res50), or not (vgg16)
+    out.append(Site("head", ("upconv1", "classifier"), lambda S, b: [(b, 32, S // h, S // h)],
+                    _vgg_head_run if half else _head_run, "head", h, loss=True))
+    return out
+
+
+def sites(model_name: str = "res50") -> list[Site]:
+    _check(model_name)
+    if model_name == "vgg16":
+        return _vgg_backbone() + _decoder(VGG_TAP_CHANNELS, half=True)
+    return _resnet_backbone() + _decoder(TAP_CHANNELS, half=False)
+
+
+def grid(model_name: str = "res50") -> list[Site]:
+    """the sites the GPU grid runs: the representative ones, without the WS-GN models' decoder (`res50`'s code at
+    `res50`'s shapes, which the `res50` rows already run)"""
+    decoder = ("trans", "sim", "upconv", "upadd", "head")
+    return [s for s in sites(model_name) if s.representative and not (model_name in WSGN and s.kind in decoder)]
+
+
+def by_name(model_name: str = "res50") -> dict[str, Site]:
+    return {s.name: s for s in sites(model_name)}
 
 
 def modules(model: nn.Module, site: Site) -> dict[str, nn.Module]:
     return {p: model.get_submodule(p) for p in site.paths}
 
 
-def owner(name: str) -> list[str]:
-    """the sites a parameter / buffer name of res50 belongs to"""
-    return [s.name for s in sites() if any(name.startswith(p + ".") for p in s.paths)]
+def owner(name: str, model_name: str = "res50") -> list[str]:
+    """the sites a parameter / buffer name of the model belongs to"""
+    return [s.name for s in sites(model_name) if any(name.startswith(p + ".") for p in s.paths)]
 
 
-def dispatch(site: Site, size: int, amp: bool) -> dict[str, bool]:
+def _grouped_conv_on_kernels(site: Site) -> bool:
+    """`wsgn.grouped_conv_on_kernels` for the ResNeXt-50 32×4d unit of `site`: its 3×3 has width / 16 channels in each
+    of its 32 groups (width 64 … 512 by stage) and stride 2 in the first unit of stages 8 … 32; the kernels take 8
+    channels per group at stride 2, so the first unit of stage 8 alone"""
+    if site.kind != "down":
+        return False
+    stride = int(site.name.split(".")[0][len("div_"):])
+    return dict((s, w) for s, w, _ in STAGES)[stride] // 16 == 8
+
+
+def dispatch(site: Site, size: int, amp: bool, model_name: str = "res50") -> dict[str, bool]:
     """backward node → present, for the engine's forward of `site` at image size `size` (amp: 16-bit shadow weights)"""
+    _check(model_name)
     hw = size // site.stride
     want = dict.fromkeys(SEAM_NODES, False)
-    if site.kind in ("stem", "pool", "down", "plain", "sim", "upconv", "head"):
+    backbone = site.kind in ("stem", "pool", "down", "plain", "vpool")
+    if site.kind in ("sim", "upconv", "head") or (backbone and model_name not in WSGN):
         want[BN] = True
+    if backbone and model_name in WSGN:
+        want[GN] = want[WS] = True   # every norm is GroupNorm(32), every convolution weight-standardised
+        want[WSG] = model_name == "wsgn_resnext50" and _grouped_conv_on_kernels(site)
     if site.kind == "pool":
         want[MAX] = True
+    if site.kind == "vpool":
+        want[MAX2] = True            # C = 64 … 512 and H, W ≥ 2 at every VGG pool
     if site.kind == "sim":
-        even = hw % 2 == 0           # avgpool2 needs even H, W; the ×2 bilinear back to hw exists only then
-        want[AVG] = want[UP] = even
-    if site.kind in ("upadd", "head"):
-        want[UP] = True
+        even = hw % 2 == 0           # avgpool2 needs even H, W; the ×2 bilinear back to hw exists only then (vgg16: at
+        want[AVG] = want[UP] = even  # strides 1 … 16 of 256² … 384² always even)
+    if site.kind == "upadd" or (site.kind == "head" and model_name != "vgg16"):
+        want[UP] = True              # vgg16's head has no ×2 up-sample
     if site.kind == "trans":
         want[CONVB] = amp            # C = 64: sod_colsum's bias gradient, reached through the shadow-weight forward
     return want                      # head: the classifier's C = 1 never takes `conv_bias`
 
 
-def stock_twin(site: Site, model: nn.Module | None = None, dtype: torch.dtype = torch.float64) -> dict[str, nn.Module]:
-    """copies of the site's modules from a stock `res50` (`nn.BatchNorm2d` as built, no amp), in `dtype` (float64 by
-    default).  `model`: the stock model to copy from, else `init_seed(0)` + `res50()`, the engine's starting point.
-    Run them with `resample.ENABLED` off (see `stock_modules`)."""
+def stock_twin(site: Site, model: nn.Module | None = None, dtype: torch.dtype = torch.float64,
+               model_name: str = "res50") -> dict[str, nn.Module]:
+    """copies of the site's modules from a stock model (`nn.BatchNorm2d`, `nn.GroupNorm` and `WSConv2d` as built, no
+    amp), in `dtype` (float64 by default).  `model`: the stock model to copy from, else `init_seed(0)` + the factory
+    `model_name`, the engine's starting point.  Run them with `resample.ENABLED` off (see `stock_modules`)."""
+    _check(model_name)
     if model is None:
         from distributed_sod_project_b200 import network
         from distributed_sod_project_b200.utils import init_seed
         init_seed(0)
-        model = network.res50()
+        model = getattr(network, model_name)()
     return {p: copy.deepcopy(m).to(dtype) for p, m in modules(model, site).items()}
 
 
@@ -160,24 +235,29 @@ class stock_modules:
         return False
 
 
-def compose(model: nn.Module, image: torch.Tensor) -> torch.Tensor:
+def compose(model: nn.Module, image: torch.Tensor, model_name: str = "res50") -> torch.Tensor:
     """`_TestModel.forward` restated site by site (every site, in model order)"""
-    table = by_name()
+    table = by_name(model_name)
 
     def run(name, *xs):
         site = table[name]
         return site.run(modules(model, site), *xs)
 
-    x = run("stem", image)
-    feats = {2: x}
-    x = run("pool+div_4.1.0", x)
-    for u in range(1, 3):
-        x = run(f"div_4.1.{u}", x)
-    feats[4] = x
-    for stride, _, units in STAGES[1:]:
-        for u in range(units):
-            x = run(f"div_{stride}.{u}", x)
-        feats[stride] = x
+    if model_name == "vgg16":
+        feats, x = {}, image
+        for s in reversed(TAPS):
+            x = feats[s] = run(f"div_{s}", x)
+    else:
+        x = run("stem", image)
+        feats = {2: x}
+        x = run("pool+div_4.1.0", x)
+        for u in range(1, 3):
+            x = run(f"div_4.1.{u}", x)
+        feats[4] = x
+        for stride, _, units in STAGES[1:]:
+            for u in range(units):
+                x = run(f"div_{stride}.{u}", x)
+            feats[stride] = x
     lat = {s: run(f"trans{s}", feats[s]) for s in (2, 4, 8, 16, 32)}
     d = None
     for s in TAPS:

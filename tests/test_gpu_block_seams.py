@@ -1,17 +1,22 @@
-"""Every block of `res50` through the engine's autograd seam, against float64 autograd of the same block.
+"""Every block of `res50`, `vgg16`, `wsgn_res50` and `wsgn_resnext50` through the engine's autograd seam, against float64
+autograd of the same block.
 
-`tests/test_gpu_model_grads.py` checks the seam (`_SyncBNFn`, `raw_backward`, `_Up2x`, `_AvgPool2x2`, `_MaxPool3x3s2`,
-`_ConvBias`, `_FusedLossFn`, the `network/blocks.py` helpers and the shadow-weight conv forward of `amp.py`) only through
-the whole model, which amplifies rounding about 10³-fold: in 16 bits a wiring fault hides there.  A single block has no
-such amplification, so here every site of oracle/block_sites.py is held close to float64 on its own.
+`tests/test_gpu_model_grads.py` and `tests/test_gpu_backbones.py` check the seam (`_SyncBNFn`, `raw_backward`, `_Up2x`,
+`_AvgPool2x2`, `_MaxPool3x3s2`, `_MaxPool2x2s2`, `_ConvBias`, `_FusedLossFn`, `_GroupNormFn`, `_WSFn`, `_WSGroupConvFn`,
+the `network/blocks.py` helpers and the shadow-weight conv forward of `amp.py`) only through the whole model, which
+amplifies rounding about 10³-fold: in 16 bits a wiring fault hides there.  A single block has no such amplification, so
+here every site of oracle/block_sites.py is held close to float64 on its own.  Rows: every representative site of each
+backbone (`bs.grid`); the WS-GN models' decoder is `res50`'s code at `res50`'s shapes and runs in the `res50` rows.
 
-* Engine: the real `Trainer` construction (`sgd_all`, SyncBN conversion, bf16 / fp16 `amp.initialize` with shadow weights
-  and a real `FusedSGD`).  Each site runs on the engine's own modules; the gradients are read where the step reads them —
+* Engine: the real `Trainer` construction (`sgd_all`, SyncBN and WS-GN conversion, bf16 / fp16 `amp.initialize` with
+  shadow weights and a real `FusedSGD`), one backbone's Trainers at a time.  Each site runs on the engine's own modules; the gradients are read where the step reads them —
   the fp32 flat `.grad`, the bound 16-bit bias views, and the stolen 16-bit weight gradients after `_gather_stolen`.
   fp16 runs with a loss scale of 2¹² (the upstream gradient is scaled, the gradients read back divided by it).
 * Reference: the site's modules copied from the stock model in float64 (`stock_twin`), run on exactly the engine's
-  operands — the input rounded to the activation dtype, conv weights and biases equal to the 16-bit shadow values, fp32
-  BN parameters — so rounding inside the block is the only difference.
+  operands — the input rounded to the activation dtype, conv weights and biases equal to the 16-bit shadow values (VGG's
+  folded backbone biases included), fp32 BN / GroupNorm parameters, the fp32 master of a WS convolution (no shadow: Ŵ is
+  rounded once inside the block, by the engine and the stock yardstick alike) — so rounding inside the block is the only
+  difference.
 * Yardstick: the same stock modules in fp32 (TF32 off, deterministic cuDNN) or under `torch.autocast`, same operands.
   Per tensor, e2 = ‖g − g64‖₂/‖g64‖₂ and emax = max|g − g64|/max|g64|, and e(engine) ≤ A·(e(stock) + median) as in
   test_gpu_model_grads.py, for the output, the input gradient(s), every parameter gradient and the running statistics;
@@ -22,11 +27,19 @@ Paths: eager training; the site captured in a CUDA graph and replayed on two fre
 the site inside `torch.utils.checkpoint` as `cp_res50` runs it (bit for bit; running statistics updated twice,
 `num_batches_tracked` + 2); eval mode with grad enabled (against float64 in eval mode).
 
-The ×2 up-sample keeps its output in the activation dtype where stock autocast returns fp32, so a 16-bit output that
-stock holds in fp32 is allowed one rounding of the activation dtype more (OUT_SLACK).  Exact where an exact answer exists:
+The ×2 up-sample and GroupNorm keep their output in the activation dtype where stock autocast returns fp32 (so the WS-GN
+bottlenecks' whole residual stream is 16-bit), so a 16-bit output that stock holds in fp32 is allowed one rounding of the
+activation dtype more (OUT_SLACK).  A ReLU decision at a pre-activation within rounding of zero goes either way; one such
+decision moves one element of a norm layer's gradient by its full size (e2 ≈ 1e-3 in a block, far above the fp32 bound),
+for the stock yardstick as for the engine.  So when the A-rule fails, each is measured again against a float64 run that
+takes its own ReLU decisions, provided every decision where the engine differs from float64 sits within TIE_REL (the
+rounding of a 4608-term fp32 sum; four roundings of the 16-bit type) of zero.  Exact where an exact answer exists:
 the two folded biases of a `pre` BN get the same Σ dz, the `trans*` bias gradient under shadow weights is `colsum(dy)`,
-a residual's gradient is the ReLU-masked dy, max-pool routes integer gradients as torch does, and the graph replay and
-the checkpointed run equal eager.
+a residual's gradient is the ReLU-masked dy (for SyncBN and GroupNorm, in its own dtype), max-pool routes integer
+gradients as torch does, GroupNorm gives the same bits for NCHW and channels-last operands, the γ/β and WS weight
+gradients are the same bits added into a bound fp32 `.grad` or returned to autograd and a second backward doubles them,
+`zero_grad` clears a backward whose only writes were the GroupNorm / WS kernels' adds, and the graph replay and the
+checkpointed run equal eager.
 
 Measured on an H100 80GB HBM3 at 700 W (S = 256, batch 2; batch 16 at 320² in bf16).  Worst ratio e(engine) /
 (e(stock) + median) over all sites and paths, against BOUND (at least 2× above):
@@ -44,9 +57,25 @@ shifted or sign-flipped gradient.  It does not clear that margin for the bf16 bo
 (0.45-0.59), nor for fp16 sim32 (0.28; other fp16 bottlenecks and SIMs 0.10-0.21): stock bf16 autograd of a training-mode
 BN block is itself 5-9 % from float64 there.  A wiring fault in those sites is caught by the fp32 and eval cases, by the
 exact checks above and by reading the gradients from the step's buffers.  The file runs in about a minute.
+
+The same measurements for the other rows (worst ratios without `upsample_add*`, whose output bound is OUT_SLACK alone):
+    vgg16           fp32 e2 4.57 emax 10.26 (div_2, eval)   bf16 0.89 / 0.97 (head, eval; bs 16 0.74 / 0.96)
+                    fp16 0.96 (head, eval) / 1.56 (sim32)
+    wsgn_res50      fp32 0.88 / 1.15 (div_4.1.1)   bf16 0.66 / 0.87 (bs 16 0.62 / 0.89)   fp16 0.65 / 0.94
+    wsgn_resnext50  fp32 1.40 / 2.23 (div_4.1.1, eval)   bf16 0.62 / 0.90 (bs 16 0.67 / 0.89)   fp16 0.68 / 0.94
+Three cases took the ReLU-decision rule: wsgn_res50 div_16.0 fp32 eager (1 decision, |pre| / max 4.6e-8), vgg16 div_16
+fp32 eval (2, 2.1e-7) and vgg16 sim32 fp16 eval (7, 7.8e-5); each then holds at ratio ≤ 0.62 / 0.85.  Median stock e2
+of the gradients (fp32 / bf16 / fp16; bf16 at 320² bs 16 within 10 % of 256² bs 2):
+    vgg16  slices 8.8e-6-7.2e-3 / 5.2-9.1e-2 / 1.8-3.3e-2   sim* ≤ 9.6e-4 / 8.2-9.6e-2 / 2.5-3.1e-2
+           trans* 2e-7 / 2.4e-3 / 3.0e-4   upconv* ≤ 4.6e-7 / 2.9-9.2e-3 / ≤ 3.6e-4   head 5.2e-7 / 1.6e-3 / 1.9e-4
+    wsgn_res50 / wsgn_resnext50  stem 2.7e-7 / 3.1-3.2e-2 / 1.1e-2   bottlenecks ≤ 1.3e-3 / 4.9-7.8e-2 / 1.4-2.8e-2
+The bound stays above 0.25 for the 16-bit cases of the same kinds of site as in res50: bf16 (eager, eval and bs 16)
+WS-GN bottlenecks 0.31-0.56, VGG slices 0.25-0.51 and VGG SIM blocks 0.27-0.59.  With the new rows the file runs in
+about two and a half minutes.
 """
 import contextlib
 import statistics
+import types
 
 import pytest
 import torch
@@ -69,10 +98,20 @@ BOUND = {_F32: (8.0, 12.0), _BF16: (2.5, 2.5), _F16: (2.5, 2.5)}
 # the ×2 up-sample stores its output in the activation dtype where stock autocast returns fp32: one rounding of it more
 OUT_SLACK = {_F32: 0.0, _BF16: 2.0 ** -8, _F16: 2.0 ** -11}
 LOSS_SLACK = {_F32: 1e-5, _BF16: 5e-3, _F16: 2.0 ** -10}
-REP = [s for s in bs.sites() if s.representative]
+# a ReLU decision may differ from float64's only at a pre-activation this close to zero, relative to the layer's largest:
+# fp32, the worst-case rounding of the longest sum in a block, K = 3·3·512 terms at u = 2⁻²⁴; 16 bits, four roundings of
+# the activation dtype (the convolution output, pre_add and residual are each stored rounded, and so is the output)
+TIE_REL = {_F32: 3 * 3 * 512 * 2.0 ** -24, _BF16: 4 * 2.0 ** -8, _F16: 4 * 2.0 ** -11}
 PRECS = [pytest.param(d, id=NAME[d]) for d in (_F32, _BF16, _F16)]
-SITES = [pytest.param(s.name, id=s.name) for s in REP]
-RESULTS: list = []               # (site, precision, path, worst e2 ratio, worst emax ratio, stock e2 median, max bound e2)
+
+
+def _row_id(model, name):
+    return name if model == "res50" else f"{model}-{name}"       # res50's ids predate the other rows
+
+
+# one row per (model, site) of the grid, grouped by model so that each backbone's Trainers are built once per test
+SITES = [pytest.param(m, s.name, id=_row_id(m, s.name)) for m in bs.MODELS for s in bs.grid(m)]
+RESULTS: list = []               # (model/site, precision, path, worst e2 ratio, worst emax ratio, stock e2 median, max bound e2)
 
 
 @contextlib.contextmanager
@@ -94,26 +133,35 @@ def _autocast(dtype):
     return torch.autocast("cuda", dtype=dtype, enabled=dtype != _F32)
 
 
+def _one_backbone(cache, model):
+    """the rows run backbone by backbone: entering another backbone's rows releases the previous one's objects"""
+    for key in [k for k in cache if k[0] != model]:
+        del cache[key]
+
+
 @pytest.fixture(scope="module")
 def engines():
-    """one Trainer per precision (built lazily), torn down with the module's global switches restored"""
+    """one Trainer per (model, precision), built lazily, those of one backbone at a time; torn down with the module's
+    global switches restored"""
     from distributed_sod_project_b200 import amp, resample
     from distributed_sod_project_b200.network import blocks
     old = resample.ENABLED, blocks.INTERPOLATE_IN_ACTIVATION_DTYPE
     cache = {}
 
-    def get(dtype):
-        if dtype not in cache:
+    def get(model, dtype):
+        if (model, dtype) not in cache:
+            _one_backbone(cache, model)
+            torch.cuda.empty_cache()
             from distributed_sod_project_b200.engine import Trainer
             with _strict(dtype):
-                tr = Trainer(model_name="res50", lr=0.0, momentum=0.0, weight_decay=0.0, optim="sgd_all", dtype=dtype,
+                tr = Trainer(model_name=model, lr=0.0, momentum=0.0, weight_decay=0.0, optim="sgd_all", dtype=dtype,
                              channels_last=True, report_items=False)
             if dtype != _F32:
                 assert tr.optimizer.flat.shadow16 is not None and tr.optimizer.flat.shadow16.dtype == dtype
-            cache[dtype] = tr
+            cache[(model, dtype)] = tr
         # the Trainers share the module switches the engine turns on
         resample.ENABLED = blocks.INTERPOLATE_IN_ACTIVATION_DTYPE = True
-        return cache[dtype]
+        return cache[(model, dtype)]
     yield get
     cache.clear()
     amp._cfg.update(enabled=False, dynamic=False, scale=1.0, good_steps=0, growth_interval=2000, owner=None, dev=None)
@@ -122,10 +170,19 @@ def engines():
 
 @pytest.fixture(scope="module")
 def stock_model():
+    """the stock model of a name (CPU, `init_seed(0)`, the engine's starting point), one backbone at a time"""
     from distributed_sod_project_b200 import network
     from distributed_sod_project_b200.utils import init_seed
-    init_seed(0)
-    return network.res50()
+    cache = {}
+
+    def get(model):
+        if (model,) not in cache:
+            _one_backbone(cache, model)
+            init_seed(0)
+            cache[(model,)] = getattr(network, model)()
+        return cache[(model,)]
+    yield get
+    cache.clear()
 
 
 # ---- running one site ---------------------------------------------------------------------------------------------
@@ -225,7 +282,9 @@ def _engine_loss(out, mask, dtype):
 
 def _twin(tr, site, stock_model, dtype, ref_dtype, bufs0):
     """stock copies of the site's modules with the engine's operands: shadow values for 16-bit conv parameters (float64
-    twin), fp32 masters otherwise (autocast rounds them to the same values), BN buffers as the engine had them"""
+    twin), fp32 masters otherwise (autocast rounds them to the same values; a WS convolution, which has no shadow,
+    standardises its fp32 master and rounds Ŵ once, in the engine and in the stock yardstick alike), BN buffers as the
+    engine had them"""
     mods = bs.stock_twin(site, stock_model, dtype=ref_dtype)
     f = tr.optimizer.flat
     eng = _site_params(tr.module, site)
@@ -282,9 +341,11 @@ def _tensors(run, with_bufs=True):
     return t
 
 
-def _yardstick(tag, eng, stk, ref, bound, out_slack=0.0):
+def _yardstick(tag, eng, stk, ref, bound, out_slack=0.0, ref_eng=None):
     """e(engine) ≤ A·(e(stock) + median e(stock)) per tensor, medians per class (output, gradients, gradients zero in
-    exact arithmetic, running statistics); returns (worst e2 ratio, worst emax ratio, median stock e2, max e2 bound)"""
+    exact arithmetic, running statistics); returns (worst e2 ratio, worst emax ratio, median stock e2, max e2 bound).
+    `ref_eng`: the float64 reference the engine is measured against, if not `ref` (see `_check_against_fp64`)"""
+    ref_eng = ref if ref_eng is None else ref_eng
     def cls(n):
         return "out" if n == "<output>" else ("stat" if n.endswith(("running_mean", "running_var")) else "grad")
     top = max(float(ref[n].double().abs().max()) for n in ref if cls(n) == "grad")
@@ -296,11 +357,11 @@ def _yardstick(tag, eng, stk, ref, bound, out_slack=0.0):
         norms[n] = ("zero" if zero else cls(n), top if zero else float(r.norm()), top if zero else mx)
     worst, med_e2, max_bound = [0.0, 0.0], 0.0, 0.0
     for k, metric in ((0, "e2"), (1, "emax")):
-        def err(run, n):
-            d = run[n].double() - ref[n].double()
+        def err(run, n, r):
+            d = run[n].double() - r[n].double()
             return (float(d.norm()) if k == 0 else float(d.abs().max())) / norms[n][1 + k]
-        es = {n: err(stk, n) for n in ref}
-        ee = {n: err(eng, n) for n in ref}
+        es = {n: err(stk, n, ref) for n in ref}
+        ee = {n: err(eng, n, ref_eng) for n in ref}
         med = {c: statistics.median([es[n] for n in ref if norms[n][0] == c]) for c in {v[0] for v in norms.values()}}
         for n in ref:
             m = med[norms[n][0]]
@@ -315,13 +376,69 @@ def _yardstick(tag, eng, stk, ref, bound, out_slack=0.0):
     return worst[0], worst[1], med_e2, max_bound
 
 
-def _check_against_fp64(tr, stock_model, site, dtype, xs, mask, dy_seed, bufs0, path, train=True, eng=None):
-    if eng is None:
+@contextlib.contextmanager
+def _relu_decisions(record=None, impose=None, margins=None, engine=False):
+    """record: receives the ReLU decisions of every norm layer with ReLU, in call order: the engine's fused norm calls'
+    y > 0 (`engine`), or the stock modules' `bn_act` pre-activation > 0.
+    impose: such a list; the stock modules' `bn_act` then applies the k-th decisions instead of its own ReLU, counts the
+    layers in `margins["layers"]` and lists in `margins["differ"]` |pre-activation| / max |pre-activation| of the layer
+    at every position where the two differ."""
+    from distributed_sod_project_b200.network import blocks
+    from distributed_sod_project_b200.syncbn import SyncBatchNorm
+    from distributed_sod_project_b200.wsgn import GroupNorm32
+    saved = {c: c.fused_forward for c in (SyncBatchNorm, GroupNorm32)}
+    bn_act = blocks.bn_act
+
+    def recording(orig):
+        def fused_forward(self, x, **kw):
+            y = orig(self, x, **kw)
+            if kw.get("relu", False):
+                record.append(y.detach() > 0)
+            return y
+        return fused_forward
+
+    def imposed(bn, x, *, relu=True, pre_add=None, residual=None):
+        pre = bn_act(bn, x, relu=False, pre_add=pre_add, residual=residual)
+        if not relu:
+            return pre
+        if impose is None:
+            record.append(pre.detach() > 0)
+            return F.relu(pre)
+        keep = impose[len(margins["layers"])]
+        margins["layers"].append(None)
+        p = pre.detach()
+        differ = keep != (p > 0)
+        margins["differ"].extend((p[differ].abs() / p.abs().max()).tolist())
+        return pre * keep
+
+    try:
+        if engine:
+            for c, f in saved.items():
+                c.fused_forward = recording(f)
+        else:
+            blocks.bn_act = imposed
+        yield
+    finally:
+        for c, f in saved.items():
+            c.fused_forward = f
+        blocks.bn_act = bn_act
+
+
+def _check_against_fp64(tr, stock_model, site, dtype, xs, mask, dy_seed, bufs0, path, train=True):
+    """the A-rule against float64.  If it fails, the engine and the stock yardstick are each measured again against a
+    float64 reference that takes their own ReLU decisions, provided every decision of the engine that differs from
+    float64's sits at a pre-activation within TIE_REL of zero.  Such a tie goes either way with the rounding: one
+    moves one element of a norm layer's gradient by its full size, an e2 of about 1/√(elements) ≈ 1e-3 in a block, far
+    above the fp32 bound, and it is as likely for the stock yardstick as for the engine."""
+    decisions, stock_decisions = [], []
+    with _relu_decisions(record=decisions, engine=True):
         eng = _engine_run(tr, site, dtype, xs, mask, dy_seed, train=train)
     _restore(tr, site, bufs0)
     ref = _stock_run(tr, site, stock_model, dtype, xs, mask, dy_seed, bufs0, torch.float64, train=train)
-    stk = _stock_run(tr, site, stock_model, dtype, xs, mask, dy_seed, bufs0, torch.float32, train=train)
-    tag = f"{site.name} {NAME[dtype]} {path}"
+    with _relu_decisions(record=stock_decisions):
+        stk = _stock_run(tr, site, stock_model, dtype, xs, mask, dy_seed, bufs0, torch.float32, train=train)
+    row = _row_id(type(tr.module).__name__, site.name)
+    tag = f"{row} {NAME[dtype]} {path}"
     assert set(eng["grads"]) == set(ref["grads"]), tag
     for r in (eng, stk):
         assert all(bool(torch.isfinite(t).all()) for t in _tensors(r).values()), f"{tag}: non-finite"
@@ -329,7 +446,23 @@ def _check_against_fp64(tr, stock_model, site, dtype, xs, mask, dy_seed, bufs0, 
         if n.endswith("num_batches_tracked"):
             assert int(eng["bufs"][n]) == int(b) == int(bufs0[n]) + (1 if train else 0), (tag, n)
     slack = OUT_SLACK[dtype] if (eng["out"].dtype != _F32 and stk["out"].dtype == _F32) else 0.0
-    w2, wm, med, mb = _yardstick(tag, _tensors(eng), _tensors(stk), _tensors(ref), BOUND[dtype], slack)
+    try:
+        w2, wm, med, mb = _yardstick(tag, _tensors(eng), _tensors(stk), _tensors(ref), BOUND[dtype], slack)
+    except AssertionError:
+        refs = []
+        for taken in (decisions, stock_decisions):
+            margins = {"layers": [], "differ": []}
+            with _relu_decisions(impose=taken, margins=margins):
+                refs.append(_stock_run(tr, site, stock_model, dtype, xs, mask, dy_seed, bufs0, torch.float64, train=train))
+            assert len(margins["layers"]) == len(taken), tag
+            if taken is decisions:
+                differ = margins["differ"]
+                assert differ and max(differ) <= TIE_REL[dtype], f"{tag}: ReLU decisions differ at |pre| / max {differ[:8]}"
+        print(f"\n{tag}: {len(differ)} ReLU decision(s) of the engine differ from float64's, at |pre-activation| / max "
+              f"<= {max(differ):.1e}")
+        tag += " (own ReLU decisions)"
+        w2, wm, med, mb = _yardstick(tag, _tensors(eng), _tensors(stk), _tensors(refs[1]), BOUND[dtype], slack,
+                                     ref_eng=_tensors(refs[0]))
     if site.kind == "sim":
         # the SyncBN backward adds the same Σ dz into both folded biases of a conv_bn_act with `pre`
         for a, b in (("h2h_1", "l2h_1"), ("l2l_1", "h2l_1"), ("h2h_2", "l2h_2")):
@@ -339,7 +472,7 @@ def _check_against_fp64(tr, stock_model, site, dtype, xs, mask, dy_seed, bufs0, 
         l64 = ref["loss"]
         assert abs(eng["loss"] - l64) <= BOUND[dtype][0] * abs(stk["loss"] - l64) + LOSS_SLACK[dtype] * abs(l64), \
             (tag, eng["loss"], stk["loss"], l64)
-    RESULTS.append((site.name, NAME[dtype], path, w2, wm, med, mb))
+    RESULTS.append((row, NAME[dtype], path, w2, wm, med, mb))
     print(f"\n{tag}: worst ratio e2 {w2:.3f} emax {wm:.3f}; stock median gradient e2 {med:.2e}; largest e2 bound {mb:.2e}")
     return eng
 
@@ -350,9 +483,9 @@ def _restore(tr, site, bufs0):
             b.copy_(bufs0[n])
 
 
-def _setup(engines, name, dtype, size=S, batch=BATCH, seed=11):
-    tr = engines(dtype)
-    site = bs.by_name()[name]
+def _setup(engines, model, name, dtype, size=S, batch=BATCH, seed=11):
+    tr = engines(model, dtype)
+    site = bs.by_name(model)[name]
     xs, mask, dy_seed = _operands(site, dtype, size, batch, seed)
     bufs0 = {n: b.clone() for n, b in _site_buffers(tr.module, site).items()}
     return tr, site, xs, mask, dy_seed, bufs0
@@ -370,10 +503,10 @@ def _equal_runs(a, b, tag):
 
 # ---- the grid ------------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("dtype", PRECS)
-@pytest.mark.parametrize("name", SITES)
-def test_eager_matches_fp64(engines, stock_model, name, dtype):
-    tr, site, xs, mask, dy_seed, bufs0 = _setup(engines, name, dtype)
-    eng = _check_against_fp64(tr, stock_model, site, dtype, xs, mask, dy_seed, bufs0, "eager")
+@pytest.mark.parametrize("model,name", SITES)
+def test_eager_matches_fp64(engines, stock_model, model, name, dtype):
+    tr, site, xs, mask, dy_seed, bufs0 = _setup(engines, model, name, dtype)
+    eng = _check_against_fp64(tr, stock_model(model), site, dtype, xs, mask, dy_seed, bufs0, "eager")
     _restore(tr, site, bufs0)
     if site.kind == "trans" and dtype != _F32:
         # the shadow-weight forward routes trans* through `conv_bias`: its bias gradient is colsum(dy) of the same dy
@@ -387,17 +520,17 @@ def test_eager_matches_fp64(engines, stock_model, name, dtype):
         assert f.view16(f.grad16, bias).dtype == dtype
 
 
-@pytest.mark.parametrize("name", SITES)
-def test_eager_bs16_320_bf16(engines, stock_model, name):
-    tr, site, xs, mask, dy_seed, bufs0 = _setup(engines, name, _BF16, size=320, batch=16, seed=29)
-    _check_against_fp64(tr, stock_model, site, _BF16, xs, mask, dy_seed, bufs0, "bs16-320")
+@pytest.mark.parametrize("model,name", SITES)
+def test_eager_bs16_320_bf16(engines, stock_model, model, name):
+    tr, site, xs, mask, dy_seed, bufs0 = _setup(engines, model, name, _BF16, size=320, batch=16, seed=29)
+    _check_against_fp64(tr, stock_model(model), site, _BF16, xs, mask, dy_seed, bufs0, "bs16-320")
     _restore(tr, site, bufs0)
 
 
 @pytest.mark.parametrize("dtype", PRECS)
-@pytest.mark.parametrize("name", SITES)
-def test_eval_mode_backward_matches_fp64(engines, stock_model, name, dtype):
-    tr, site, xs, mask, dy_seed, bufs0 = _setup(engines, name, dtype, seed=13)
+@pytest.mark.parametrize("model,name", SITES)
+def test_eval_mode_backward_matches_fp64(engines, stock_model, model, name, dtype):
+    tr, site, xs, mask, dy_seed, bufs0 = _setup(engines, model, name, dtype, seed=13)
     if bufs0:       # non-trivial running statistics, so the eval forward differs from the batch-statistics one
         g = torch.Generator(device="cuda").manual_seed(3)
         with torch.no_grad():
@@ -409,16 +542,16 @@ def test_eval_mode_backward_matches_fp64(engines, stock_model, name, dtype):
         shifted = {n: b.clone() for n, b in _site_buffers(tr.module, site).items()}
     else:
         shifted = bufs0
-    eng = _check_against_fp64(tr, stock_model, site, dtype, xs, mask, dy_seed, shifted, "eval", train=False)
+    eng = _check_against_fp64(tr, stock_model(model), site, dtype, xs, mask, dy_seed, shifted, "eval", train=False)
     for n, b in eng["bufs"].items():
         assert torch.equal(b, shifted[n]), f"{name}: eval changed {n}"
     _restore(tr, site, bufs0)
 
 
 @pytest.mark.parametrize("dtype", PRECS)
-@pytest.mark.parametrize("name", SITES)
-def test_checkpoint_equals_eager(engines, name, dtype):
-    tr, site, xs, mask, dy_seed, bufs0 = _setup(engines, name, dtype, seed=17)
+@pytest.mark.parametrize("model,name", SITES)
+def test_checkpoint_equals_eager(engines, model, name, dtype):
+    tr, site, xs, mask, dy_seed, bufs0 = _setup(engines, model, name, dtype, seed=17)
     eager = _engine_run(tr, site, dtype, xs, mask, dy_seed)
     with torch.no_grad(), _strict(dtype), _autocast(dtype):
         site.run(bs.modules(tr.module, site), *xs)            # the recompute's second statistics update
@@ -434,10 +567,10 @@ def test_checkpoint_equals_eager(engines, name, dtype):
 
 
 @pytest.mark.parametrize("dtype", PRECS)
-@pytest.mark.parametrize("name", SITES)
-def test_graph_replay_equals_eager(engines, name, dtype):
+@pytest.mark.parametrize("model,name", SITES)
+def test_graph_replay_equals_eager(engines, model, name, dtype):
     from distributed_sod_project_b200 import syncbn
-    tr, site, xs, mask, dy_seed, bufs0 = _setup(engines, name, dtype, seed=19)
+    tr, site, xs, mask, dy_seed, bufs0 = _setup(engines, model, name, dtype, seed=19)
     model, opt = tr.module, tr.optimizer
     mods = bs.modules(model, site)
     scale = FP16_SCALE if dtype == _F16 else 1.0
@@ -505,7 +638,7 @@ def test_graph_replay_equals_eager(engines, name, dtype):
                 leaf.grad = g
             rep = dict(out=out_g.detach(), dx=[x.grad.double() / scale for x in static], grads=_read_grads(tr, site, scale),
                        loss=None if loss_g is None else float(loss_g))
-            _equal_runs(rep, eager, f"{name} {NAME[dtype]} graph replay {k}")
+            _equal_runs(rep, eager, f"{_row_id(model, name)} {NAME[dtype]} graph replay {k}")
             for n, b in _site_buffers(model, site).items():
                 assert torch.equal(b, eager["bufs"][n]), f"{name} replay {k}: {n}"
     del graph
@@ -526,10 +659,10 @@ def _walk(fn):
 
 
 @pytest.mark.parametrize("size", bs.SIZES)
-@pytest.mark.parametrize("dtype", [pytest.param(_F32, id="fp32"), pytest.param(_BF16, id="bf16")])
-def test_dispatch_matches_site_table(engines, size, dtype):
-    tr = engines(dtype)
-    for site in REP:
+@pytest.mark.parametrize("model,dtype", [pytest.param(m, d, id=_row_id(m, NAME[d])) for m in bs.MODELS for d in (_F32, _BF16)])
+def test_dispatch_matches_site_table(engines, model, size, dtype):
+    tr = engines(model, dtype)
+    for site in bs.grid(model):
         bufs0 = {n: b.clone() for n, b in _site_buffers(tr.module, site).items()}
         xs, mask, _ = _operands(site, dtype, size, 1, 5)
         xs = [x.requires_grad_(ok) for x, ok in zip(xs, site.input_grad)]
@@ -538,9 +671,9 @@ def test_dispatch_matches_site_table(engines, size, dtype):
         if site.loss:
             out, _ = _engine_loss(out, mask, dtype)[1], None
         names = _walk(out.grad_fn)
-        want = bs.dispatch(site, size, amp=dtype != _F32)
+        want = bs.dispatch(site, size, dtype != _F32, model)
         for node, present in want.items():
-            assert (node in names) == present, (site.name, size, NAME[dtype], node, sorted(names))
+            assert (node in names) == present, (model, site.name, size, NAME[dtype], node, sorted(names))
         assert (bs.LOSS in names) == site.loss
         _restore(tr, site, bufs0)
 
@@ -802,6 +935,250 @@ def test_zero_grad_clears_a_folded_bias_only_backward(dtype):
         opt.zero_grad()
         model(x).backward(dy)
         assert torch.equal(bias_grad(), once), "stale folded-bias gradient survived zero_grad"
+    finally:
+        amp._cfg.update(enabled=False, dynamic=False, scale=1.0, good_steps=0, growth_interval=2000, owner=None, dev=None)
+
+
+# ---- seam cases on one GroupNorm32 and the weight-standardised convolutions -------------------------------------------
+def _gn(c, seed=0):
+    from distributed_sod_project_b200.wsgn import GroupNorm32
+    g = torch.Generator().manual_seed(seed)
+    gn = GroupNorm32(32, c).cuda()
+    with torch.no_grad():
+        gn.weight.copy_(torch.rand(c, generator=g) + 0.5)
+        gn.bias.copy_(torch.randn(c, generator=g) * 0.2)
+    return gn
+
+
+def _ref_gn(x, res, gn, relu):
+    """float64 autograd of act(GroupNorm(32)(x) + res), res rounded to x's dtype first as the kernel takes it"""
+    xx = x.detach().double().requires_grad_()
+    w, b = gn.weight.detach().double().requires_grad_(), gn.bias.detach().double().requires_grad_()
+    y = F.group_norm(xx, 32, w, b, gn.eps)
+    if res is not None:
+        y = y + res.detach().to(x.dtype).double()
+    return (F.relu(y) if relu else y), xx, w, b
+
+
+_GN_TOL = {_F32: 1e-5, _BF16: 2e-2, _F16: 4e-3}
+
+
+@pytest.mark.parametrize("x_dtype,res_dtype", [
+    pytest.param(d, r, id=f"x_{NAME[d]}-res_{NAME[r]}")
+    for d, r in ((_F32, _F32), (_BF16, _BF16), (_F16, _F16), (_BF16, _F32), (_F16, _F32), (_F32, _BF16))])
+def test_groupnorm_residual_gradient_is_the_masked_upstream(x_dtype, res_dtype):
+    """GroupNorm32 with the bottleneck's residual and ReLU: the output is in x's dtype (the residual rounded to it once on
+    entry); the residual's gradient is exactly the ReLU-masked upstream, handed back in the residual's own dtype.  Output,
+    dx, dγ and dβ against float64."""
+    gn = _gn(64, 1)
+    x = _t((4, 64, 8, 8), x_dtype, 20).requires_grad_()
+    res = _t((4, 64, 8, 8), res_dtype, 21).requires_grad_()
+    y = gn.fused_forward(x, residual=res, relu=True)
+    assert y.dtype == x_dtype and type(y.grad_fn).__name__ == bs.GN
+    dy = _t(y.shape, x_dtype, 22)
+    y.backward(dy)
+    assert res.grad.dtype == res_dtype
+    assert torch.equal(res.grad, (dy * (y > 0)).to(res_dtype))
+    y64, x64, w64, b64 = _ref_gn(x, res, gn, relu=True)
+    y64.backward(dy.double())
+    tol = _GN_TOL[x_dtype]
+    _close(y, y64, tol, "output")
+    _close(x.grad, x64.grad, tol, "dx")
+    _close(gn.weight.grad, w64.grad, max(tol, 1e-4), "dgamma")
+    _close(gn.bias.grad, b64.grad, max(tol, 1e-4), "dbeta")
+
+
+@pytest.mark.parametrize("scale", [pytest.param(2.0 ** -6, id="var_2e-4"), pytest.param(2.0 ** -10, id="var_1e-6")])
+@pytest.mark.parametrize("dtype", [pytest.param(_F32, id="fp32"), pytest.param(_BF16, id="bf16")])
+def test_groupnorm_takes_the_module_eps(dtype, scale):
+    """at a group variance near eps (x of std 2⁻⁶ and 2⁻¹⁰ against eps = 1e-5) the output and every gradient depend on
+    eps at first order: GroupNorm32 against float64 GroupNorm with the module's eps"""
+    gn = _gn(64, 7)
+    x = (_t((4, 64, 8, 8), _F32, 35) * scale).to(dtype).detach().requires_grad_()
+    y = gn.fused_forward(x)
+    dy = _t(y.shape, dtype, 36)
+    y.backward(dy)
+    y64, x64, w64, b64 = _ref_gn(x, None, gn, relu=False)
+    y64.backward(dy.double())
+    tol = _GN_TOL[dtype]
+    _close(y, y64, tol, "output")
+    _close(x.grad, x64.grad, tol, "dx")
+    _close(gn.weight.grad, w64.grad, max(tol, 1e-4), "dgamma")
+    _close(gn.bias.grad, b64.grad, max(tol, 1e-4), "dbeta")
+
+
+def test_groupnorm_layouts_give_identical_results():
+    """NCHW-contiguous and sliced (non-contiguous) x, residual and dy are converted on entry: the GroupNorm results equal
+    the channels-last run bit for bit"""
+    gn = _gn(64, 2)
+    dtype = _BF16
+    big = _t((4, 64, 12, 12), dtype, 26, cl=False)
+    big_res = _t((4, 64, 12, 12), dtype, 27, cl=False)
+    dy_cl = _t((4, 64, 10, 12), dtype, 28)
+
+    def views(t):
+        return {"channels_last": t[:, :, 1:-1, :].contiguous(memory_format=torch.channels_last),
+                "nchw": t[:, :, 1:-1, :].contiguous(), "sliced": t.detach().clone()[:, :, 1:-1, :]}
+    assert not views(big)["sliced"].is_contiguous(memory_format=torch.channels_last)
+    out = {}
+    for name in ("channels_last", "nchw", "sliced"):
+        for dyn, dy in (("dy_cl", dy_cl), ("dy_nchw", dy_cl.contiguous())):
+            x, res = views(big)[name].requires_grad_(), views(big_res)[name].requires_grad_()
+            gn.weight.grad = gn.bias.grad = None
+            y = gn.fused_forward(x, residual=res, relu=True)
+            y.backward(dy)
+            out[(name, dyn)] = (y.detach(), x.grad, res.grad, gn.weight.grad.clone(), gn.bias.grad.clone())
+    ref = out[("channels_last", "dy_cl")]
+    for k, v in out.items():
+        for a, b in zip(v, ref):
+            assert torch.equal(a.contiguous(), b.contiguous()), k
+
+
+@pytest.mark.parametrize("mode", ["direct", "gamma_frozen", "beta_frozen", "both_frozen"])
+def test_groupnorm_param_grad_paths_and_second_backward(mode):
+    """γ/β gradients the kernel adds into bound fp32 .grad buffers (as the fused optimizers bind them) equal, bit for bit,
+    those it hands back to autograd; with γ, β or both frozen the trainable one comes back through autograd into its
+    bound .grad and a frozen one's stays untouched.  A second backward without zeroing doubles every gradient exactly."""
+    c, dtype = 64, _BF16
+    x0, res0, dy = _t((4, c, 16, 8), dtype, 23), _t((4, c, 16, 8), dtype, 24), _t((4, c, 16, 8), dtype, 25)
+
+    def run(gn, k):
+        x, res = x0.detach().clone().requires_grad_(), res0.detach().clone().requires_grad_()
+        runs = []
+        for _ in range(k):
+            y = gn.fused_forward(x, residual=res, relu=True)
+            y.backward(dy)
+            runs.append({"y": y.detach(), "dx": x.grad.clone(), "dres": res.grad.clone(),
+                         "dw": None if gn.weight.grad is None else gn.weight.grad.clone(),
+                         "db": None if gn.bias.grad is None else gn.bias.grad.clone()})
+        return runs
+
+    from distributed_sod_project_b200 import _lib
+    ref = run(_gn(c, 6), 1)[0]                                  # both trainable, nothing bound: returned to autograd
+    y64, x64, w64, b64 = _ref_gn(x0, res0, _gn(c, 6), relu=True)
+    y64.backward(dy.double())
+    _close(ref["dw"], w64.grad, 2e-2, "dgamma")
+    _close(ref["db"], b64.grad, 2e-2, "dbeta")
+    gn = _gn(c, 6)
+    gn.weight.requires_grad_(mode not in ("gamma_frozen", "both_frozen"))
+    gn.bias.requires_grad_(mode not in ("beta_frozen", "both_frozen"))
+    for p in (gn.weight, gn.bias):
+        p.grad = torch.zeros_like(p)
+    writes = _lib.grad_writes
+    first, second = run(gn, 2)
+    assert (_lib.grad_writes > writes) == (mode == "direct")
+    for key, p in (("dw", gn.weight), ("db", gn.bias)):
+        if p.requires_grad:
+            assert torch.equal(first[key], ref[key]), key
+            assert torch.equal(second[key], 2 * ref[key]), key                   # fp32: g + g is exact
+        else:
+            assert float(first[key].abs().max()) == 0.0 and float(second[key].abs().max()) == 0.0, key
+    for key in ("y", "dx", "dres"):
+        assert torch.equal(first[key], ref[key]), key
+    assert torch.equal(second["dx"], 2 * ref["dx"]) and torch.equal(second["dres"], 2 * ref["dres"])
+
+
+def _fused_ws(cin, cout, stride, groups, seed):
+    from distributed_sod_project_b200 import wsgn
+    from distributed_sod_project_b200.network.blocks import WSConv2d
+    torch.manual_seed(seed)
+    conv = WSConv2d(cin, cout, 3, stride, 1, groups=groups, bias=False).cuda().to(memory_format=torch.channels_last)
+    return wsgn.convert_wsgn_model(conv)
+
+
+@pytest.mark.parametrize("bound", [pytest.param(False, id="returned"), pytest.param(True, id="bound")])
+@pytest.mark.parametrize("groups", [pytest.param(1, id="ws"), pytest.param(32, id="ws_gconv")])
+def test_ws_weight_grad_paths_and_second_backward(groups, bound):
+    """the weight gradient of a WS convolution (`_WSFn` after cuDNN; `_WSGroupConvFn` for the 32-group 3×3 on the
+    kernels) is the same bit for bit whether the kernel adds it into a bound fp32 .grad or returns it to autograd, close to
+    float64, and a second backward without zeroing doubles it exactly"""
+    from distributed_sod_project_b200 import _lib
+    c = 256 if groups > 1 else 64                           # 8 channels per group at stride 2: csrc/gconv.cu
+    conv = _fused_ws(c, c, 2, groups, 30)
+    x0, dtype = _t((2, c, 16, 12), _BF16, 31), _BF16
+
+    def run(k, bind):
+        conv.weight.grad = torch.zeros_like(conv.weight) if bind else None
+        x = x0.detach().clone().requires_grad_()
+        runs = []
+        for _ in range(k):
+            with torch.autocast("cuda", dtype=dtype):
+                y = conv(x)
+            names = _walk(y.grad_fn)
+            assert (bs.WSG in names) == (groups > 1) and (bs.WS in names) == (groups == 1), names
+            y.backward(_t(y.shape, dtype, 32))
+            runs.append((x.grad.clone(), conv.weight.grad.clone()))
+        return runs
+
+    writes = _lib.grad_writes
+    (dx_ref, dw_ref), = run(1, False)
+    assert _lib.grad_writes == writes                       # nothing bound: returned to autograd
+    (dx1, dw1), (dx2, dw2) = run(2, bound)                  # unbound: autograd's .grad is bound from the second on
+    assert _lib.grad_writes > writes
+    assert torch.equal(dx1, dx_ref) and torch.equal(dw1, dw_ref)
+    assert torch.equal(dx2, 2 * dx_ref) and torch.equal(dw2, 2 * dw_ref)
+    assert dw1.dtype == torch.float32
+    # float64: the same x and dy through the stock WSConv2d
+    w64 = conv.weight.detach().double().requires_grad_()
+    wt = types.SimpleNamespace(weight=w64, eps=conv.eps)
+    y64 = F.conv2d(x0.double(), type(conv).standardized_weight(wt), None, 2, 1, 1, groups)
+    y64.backward(_t(y64.shape, dtype, 32).double())
+    _close(dw1, w64.grad, 2e-2, "dW")
+
+
+class _WSGN(nn.Module):
+    def __init__(self):
+        super().__init__()
+        from distributed_sod_project_b200.network.blocks import WSConv2d
+        self.conv = WSConv2d(16, 64, 3, 1, 1, bias=False)
+        self.gn = nn.GroupNorm(32, 64)
+
+    def forward(self, x):
+        from distributed_sod_project_b200.network.blocks import bn_act
+        return bn_act(self.gn, self.conv(x))
+
+
+@pytest.mark.parametrize("trains", ["gn", "ws", "both"])
+@pytest.mark.parametrize("dtype", [pytest.param(_F32, id="fp32"), pytest.param(_BF16, id="bf16")])
+def test_zero_grad_clears_a_groupnorm_or_ws_only_backward(dtype, trains):
+    """a backward whose only gradient writes are the GroupNorm and / or WS kernels' adds into the bound fp32 .grad
+    (input without gradient; the other module frozen): after a step, such a backward and zero_grad, the next backward
+    must see a clean buffer"""
+    from distributed_sod_project_b200 import amp, wsgn
+    from distributed_sod_project_b200.optim import make_optimizer
+    from distributed_sod_project_b200.syncbn import convert_syncbn_model
+    torch.manual_seed(1)
+    model = _WSGN().cuda().to(memory_format=torch.channels_last)
+    with torch.no_grad():
+        model.gn.weight.uniform_(0.5, 1.5)
+        model.gn.bias.normal_(0, 0.2)
+    if trains == "ws":
+        model.gn.requires_grad_(False)
+    if trains == "gn":
+        model.conv.requires_grad_(False)
+    opt = make_optimizer(model, "sgd_all", dict(lr=0.0, momentum=0.0, weight_decay=0.0))
+    model = wsgn.convert_wsgn_model(convert_syncbn_model(model))
+    try:
+        if dtype != _F32:
+            model, opt = amp.initialize(model, opt, opt_level="O1", dtype=dtype)
+        params = [p for p in model.parameters() if p.requires_grad]
+        assert params
+
+        def grads():
+            return [p.grad.clone() for p in params]
+
+        x = _t((4, 16, 8, 8), dtype, 33)
+        dy = _t((4, 64, 8, 8), dtype, 34)
+        opt.zero_grad()
+        model(x).backward(dy)
+        once = grads()
+        assert all(float(g.abs().max()) > 0 for g in once)
+        opt.step()
+        model(x).backward(dy)                           # after the step: writes only the kernels' adds make
+        opt.zero_grad()
+        model(x).backward(dy)
+        for g, g1 in zip(grads(), once):
+            assert torch.equal(g, g1), "stale GroupNorm / WS gradient survived zero_grad"
     finally:
         amp._cfg.update(enabled=False, dynamic=False, scale=1.0, good_steps=0, growth_interval=2000, owner=None, dev=None)
 
