@@ -12,7 +12,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libsod_b200.so")
 OBJDIR = os.path.join(HERE, "build")
 STAMP = os.path.join(OBJDIR, "arch.txt")   # the target LIB was built for: a library for another target is rebuilt
-SOURCES = ("api.cu", "loss.cu", "sgd.cu", "syncbn.cu", "resample.cu", "maxpool.cu", "pipeline.cu", "resize.cu", "augment.cu", "joint.cu", "wfm.cu", "wsgn.cu", "gconv.cu")
+SOURCES = ("api.cu", "loss.cu", "sgd.cu", "syncbn.cu", "resample.cu", "nearest.cu", "maxpool.cu", "pipeline.cu", "resize.cu", "augment.cu", "joint.cu", "wfm.cu", "wsgn.cu", "gconv.cu")
 ARCH = ("-gencode", "arch=compute_90a,code=sm_90a")
 NVCC_FLAGS = (
     *ARCH, "-O3", "-lineinfo", "-std=c++17",

@@ -4,7 +4,7 @@ Written from scratch for this repo; the *contract* it keeps is the reference's
 (lartpang/Distributed-SOD-Project):
 
 * parameter / buffer names and registration order of `network/TestModel.py:17-185`,
-  `module/BaseBlocks.py:10-40`, `module/MyLightModule.py:11-54`,
+  `module/BaseBlocks.py:10-40`, `module/MyLightModule.py:11-236`,
   `backbone/origin/resnet.py:61-156`, `backbone/origin/from_origin.py:7-15`
   (so reference checkpoints load, and `make_optimizer("f3_trick")` groups by the same
   `div_2` / `div*` prefixes, `utils/pipeline_ops.py:295-303`);
@@ -67,6 +67,23 @@ def conv_bn_act(conv: nn.Conv2d, bn: nn.Module, x: torch.Tensor, *, relu: bool =
     return bn_act(bn, conv(x), relu=relu, pre_add=None if pre is None else pre[0](pre[1]), residual=residual)
 
 
+def conv3_bn_act(conv: nn.Conv2d, bn: nn.Module, x: torch.Tensor, pre, pre2) -> torch.Tensor:
+    """y = relu( BN( conv(x) + pre_conv(pre_x) + pre2_conv(pre2_x) ) ), summed left to right as the reference does
+    (`bnm_1(h2m + m2m + l2m)`, module/MyLightModule.py:202,209).
+
+    The SyncBN kernel takes one pre-add and two folded biases, so on the engine the second and third operands are joined
+    by one add into `pre_add`, and their biases by one add into the second `conv_bias` slot; autograd hands that slot's
+    gradient Σ dz to both biases."""
+    fused = getattr(bn, "fused_forward", None)
+    if fused is not None and x.is_cuda:
+        a, b1 = _conv_nobias(conv, x)
+        p, b2 = _conv_nobias(pre[0], pre[1])
+        q, b3 = _conv_nobias(pre2[0], pre2[1])
+        b23 = b3 if b2 is None else (b2 if b3 is None else b2 + b3)
+        return fused(a, pre_add=p + q, relu=True, conv_bias=(b1, b23))
+    return bn_act(bn, conv(x) + pre[0](pre[1]) + pre2[0](pre2[1]), relu=True)
+
+
 # torch.autocast lists upsample_bilinear2d as an fp32 op: under bf16 autocast every interpolate becomes
 # cast-up → fp32 kernel → fp32 result that then drags the following adds into fp32 (≈2 ms of casts per iteration on
 # the TestModel).  The engine sets this flag so the interpolation runs natively in the activation dtype
@@ -100,6 +117,17 @@ def avgpool2(pool: nn.Module, x: torch.Tensor) -> torch.Tensor:
         if y is not None:
             return y
     return pool(x)
+
+
+def nearest2x(x: torch.Tensor) -> torch.Tensor:
+    """`nn.Upsample(scale_factor=2, mode="nearest")` of LightAIM (module/MyLightModule.py:64,146); on the engine the
+    channels-last kernel, in x's dtype"""
+    if x.is_cuda:
+        from .. import resample
+        y = resample.upsample2x_nearest(x)
+        if y is not None:
+            return y
+    return F.interpolate(x, scale_factor=2, mode="nearest")
 
 
 def upsample_add(*feats: torch.Tensor) -> torch.Tensor:
@@ -345,3 +373,98 @@ class SIM(nn.Module):
         l_new = conv_bn_act(self.l2l_1, self.bnl_1, xl, pre=(self.h2l_1, down(xh)))
         # stage 2: merge to full-res
         return conv_bn_act(self.h2h_2, self.bnh_2, h_new, pre=(self.l2h_2, bilinear(l_new, size=hw)))
+
+
+class _Neck(nn.Module):
+    """A LightAIM block (reference module/MyLightModule.py:57-213): built from a (name, in, out) table in the reference's
+    registration order, 3x3 convolutions except the 1x1 `identity`, torch's default init.  Channel keys are resolved
+    through `ch`; a None input marks a BatchNorm."""
+
+    def _build(self, layout, ch):
+        self.pool = nn.AvgPool2d((2, 2), stride=2)       # h2l_pool / downsample: no parameters, not part of the state
+        for name, src, dst in layout:
+            if src is None:
+                self.add_module(name, nn.BatchNorm2d(ch[dst]))
+            elif name == "identity":
+                self.add_module(name, nn.Conv2d(ch[src], ch[dst], 1))
+            else:
+                self.add_module(name, nn.Conv2d(ch[src], ch[dst], 3, 1, 1))
+
+    def down(self, t):
+        return avgpool2(self.pool, t)
+
+
+class Conv2nV1(_Neck):
+    """`conv_2nV1` (module/MyLightModule.py:57-140): a high- and a low-resolution stream (mid_c = min(in_hc, in_lc)
+    channels), one cross exchange, and a merge into the `main` stream (0: high, 1: low) with a 1x1 identity shortcut."""
+
+    _HEAD = (("h2h_0", "h", "m"), ("l2l_0", "l", "m"), ("bnh_0", None, "m"), ("bnl_0", None, "m"),
+             ("h2h_1", "m", "m"), ("h2l_1", "m", "m"), ("l2h_1", "m", "m"), ("l2l_1", "m", "m"),
+             ("bnl_1", None, "m"), ("bnh_1", None, "m"))
+    _MAIN = {0: (("h2h_2", "m", "m"), ("l2h_2", "m", "m"), ("bnh_2", None, "m"), ("h2h_3", "m", "o"), ("bnh_3", None, "o"),
+                 ("identity", "h", "o")),
+             1: (("h2l_2", "m", "m"), ("l2l_2", "m", "m"), ("bnl_2", None, "m"), ("l2l_3", "m", "o"), ("bnl_3", None, "o"),
+                 ("identity", "l", "o"))}
+
+    def __init__(self, in_hc: int, in_lc: int, out_c: int, main: int):
+        super().__init__()
+        if main not in self._MAIN:
+            raise ValueError(f"main must be 0 or 1, got {main}")
+        self.main = main
+        self._build(self._HEAD + self._MAIN[main], {"h": in_hc, "l": in_lc, "m": min(in_hc, in_lc), "o": out_c})
+
+    def forward(self, in_h, in_l):
+        h = conv_bn_act(self.h2h_0, self.bnh_0, in_h)
+        l = conv_bn_act(self.l2l_0, self.bnl_0, in_l)  # noqa: E741
+        h1 = conv_bn_act(self.h2h_1, self.bnh_1, h, pre=(self.l2h_1, nearest2x(l)))
+        l1 = conv_bn_act(self.l2l_1, self.bnl_1, l, pre=(self.h2l_1, self.down(h)))
+        if self.main == 0:
+            fuse = conv_bn_act(self.h2h_2, self.bnh_2, h1, pre=(self.l2h_2, nearest2x(l1)))
+            return conv_bn_act(self.h2h_3, self.bnh_3, fuse, residual=self.identity(in_h))
+        fuse = conv_bn_act(self.h2l_2, self.bnl_2, self.down(h1), pre=(self.l2l_2, l1))
+        return conv_bn_act(self.l2l_3, self.bnl_3, fuse, residual=self.identity(in_l))
+
+
+class Conv3nV1(_Neck):
+    """`conv_3nV1` (module/MyLightModule.py:143-213): high, middle and low streams of 64 channels, one three-way
+    exchange, and a merge into the middle stream with a 1x1 identity shortcut."""
+
+    _LAYOUT = (("h2h_0", "h", "m"), ("m2m_0", "mi", "m"), ("l2l_0", "l", "m"),
+               ("bnh_0", None, "m"), ("bnm_0", None, "m"), ("bnl_0", None, "m"),
+               ("h2h_1", "m", "m"), ("h2m_1", "m", "m"), ("m2h_1", "m", "m"), ("m2m_1", "m", "m"), ("m2l_1", "m", "m"),
+               ("l2m_1", "m", "m"), ("l2l_1", "m", "m"), ("bnh_1", None, "m"), ("bnm_1", None, "m"), ("bnl_1", None, "m"),
+               ("h2m_2", "m", "m"), ("l2m_2", "m", "m"), ("m2m_2", "m", "m"), ("bnm_2", None, "m"),
+               ("m2m_3", "m", "o"), ("bnm_3", None, "o"), ("identity", "mi", "o"))
+
+    def __init__(self, in_hc: int, in_mc: int, in_lc: int, out_c: int):
+        super().__init__()
+        self._build(self._LAYOUT, {"h": in_hc, "mi": in_mc, "l": in_lc, "m": 64, "o": out_c})
+
+    def forward(self, in_h, in_m, in_l):
+        h = conv_bn_act(self.h2h_0, self.bnh_0, in_h)
+        m = conv_bn_act(self.m2m_0, self.bnm_0, in_m)
+        l = conv_bn_act(self.l2l_0, self.bnl_0, in_l)  # noqa: E741
+        h1 = conv_bn_act(self.h2h_1, self.bnh_1, h, pre=(self.m2h_1, nearest2x(m)))
+        m1 = conv3_bn_act(self.h2m_1, self.bnm_1, self.down(h), (self.m2m_1, m), (self.l2m_1, nearest2x(l)))
+        l1 = conv_bn_act(self.m2l_1, self.bnl_1, self.down(m), pre=(self.l2l_1, l))
+        m2 = conv3_bn_act(self.h2m_2, self.bnm_2, self.down(h1), (self.m2m_2, m1), (self.l2m_2, nearest2x(l1)))
+        return conv_bn_act(self.m2m_3, self.bnm_3, m2, residual=self.identity(in_m))
+
+
+class LightAIM(nn.Module):
+    """The MINet neck (module/MyLightModule.py:216-236): five blocks, each mixing a backbone tap with its neighbours,
+    `conv0` … `conv4` from the finest stride to the coarsest.  Returns the five laterals, finest first."""
+
+    def __init__(self, iC_list, oC_list):  # noqa: N803  (the reference's argument names)
+        super().__init__()
+        ic0, ic1, ic2, ic3, ic4 = iC_list
+        oc0, oc1, oc2, oc3, oc4 = oC_list
+        self.conv0 = Conv2nV1(ic0, ic1, oc0, main=0)
+        self.conv1 = Conv3nV1(ic0, ic1, ic2, oc1)
+        self.conv2 = Conv3nV1(ic1, ic2, ic3, oc2)
+        self.conv3 = Conv3nV1(ic2, ic3, ic4, oc3)
+        self.conv4 = Conv2nV1(ic3, ic4, oc4, main=1)
+
+    def forward(self, x2, x4, x8, x16, x32):
+        return (self.conv0(x2, x4), self.conv1(x2, x4, x8), self.conv2(x4, x8, x16), self.conv3(x8, x16, x32),
+                self.conv4(x16, x32))

@@ -5,7 +5,9 @@
 (`Backbone_ResNeXt50_in3`, built as `l_resnext50(pretrained, baseWidth=4, cardinality=32)`: the reference's builder
 omits those two arguments, and its X-50-GN-WS release is 32×4d), and
 `vgg16` / `cp_vgg16`: the same decoder on the reference's VGG16-BN (`backbone.origin.from_origin.Backbone_VGG16_in3`), whose
-five slices carry 64 … 512 channels at strides 1 … 16.
+five slices carry 64 … 512 channels at strides 1 … 16, and
+`aim_res50` / `cp_aim_res50`: `res50` with MINet's LightAIM neck (module/MyLightModule.py:216-236) in place of the five
+`trans*` convolutions.
 
 Zero-arg factories looked up by name from `user_config["model"]` (reference train.py:141):
 ResNet-50 encoder → five 1×1 "trans" convs to 64 ch → top-down decoder of SIM + ConvBNReLU with
@@ -21,8 +23,8 @@ import torch
 import torch.nn as nn
 from torch.utils.checkpoint import checkpoint
 
-from .blocks import (SIM, VGG16_SLICES, ConvBNReLU, WSConv2d, bilinear, group_norm32, resnet50_stages, upsample_add,
-                     vgg16_bn_slices)
+from .blocks import (SIM, VGG16_SLICES, ConvBNReLU, LightAIM, WSConv2d, bilinear, group_norm32, resnet50_stages,
+                     upsample_add, vgg16_bn_slices)
 
 _TAPS = (32, 16, 8, 4, 2)                       # encoder strides tapped, deepest first
 _TAP_CHANNELS = {32: 2048, 16: 1024, 8: 512, 4: 256, 2: 64}
@@ -36,14 +38,18 @@ class _TestModel(nn.Module):
     def __init__(self):
         super().__init__()
         self.div_2, self.div_4, self.div_8, self.div_16, self.div_32 = self.backbone()
-        for s in _TAPS:
-            setattr(self, f"trans{s}", nn.Conv2d(self.tap_channels[s], 64, 1, 1))
+        self._build_neck()
         for s in _TAPS:
             setattr(self, f"sim{s}", SIM(64, 32))
         for s in _TAPS:
             setattr(self, f"upconv{s}", ConvBNReLU(64, 32 if s == 2 else 64, 3, 1, 1))
         self.upconv1 = ConvBNReLU(32, 32, 3, 1, 1)
         self.classifier = nn.Conv2d(32, 1, 1)
+
+    def _build_neck(self):
+        """the five 1x1 convolutions from each backbone tap to the decoder's 64 channels, deepest first"""
+        for s in _TAPS:
+            setattr(self, f"trans{s}", nn.Conv2d(self.tap_channels[s], 64, 1, 1))
 
     # -- segments (each is one checkpoint unit in cp_res50) -------------------------------------
     def _encode(self, stride: int, x):
@@ -137,6 +143,31 @@ class vgg16(_TestModel):
 
 class cp_vgg16(vgg16):
     """Activation-checkpointed twin of `vgg16`, with the same twelve segments as `cp_res50`."""
+
+    recompute = True
+
+
+class aim_res50(_TestModel):
+    """`res50` with MINet's LightAIM neck (reference module/MyLightModule.py:216-236) in place of the five 1x1 `trans*`
+    convolutions, as MINet_Res50 builds it: `trans = LightAIM((64, 256, 512, 1024, 2048), (64,) * 5)`.  The decoder
+    and head are `res50`'s.  The neck's nearest ×2 up-samples only line up with the ResNet maps when both input sides
+    are multiples of 32."""
+
+    def _build_neck(self):
+        self.trans = LightAIM(iC_list=(64, 256, 512, 1024, 2048), oC_list=(64, 64, 64, 64, 64))
+
+    def _project(self, f2, f4, f8, f16, f32):
+        return self.trans(f2, f4, f8, f16, f32)
+
+    def forward(self, image: torch.Tensor) -> torch.Tensor:
+        if image.dim() != 4 or image.shape[2] % 32 or image.shape[3] % 32:
+            raise ValueError(f"{type(self).__name__} needs input sides that are multiples of 32, got "
+                             f"{tuple(image.shape[2:])}")
+        return super().forward(image)
+
+
+class cp_aim_res50(aim_res50):
+    """Activation-checkpointed twin of `aim_res50`: the whole neck is one segment, as `cp_res50`'s `_project` is."""
 
     recompute = True
 

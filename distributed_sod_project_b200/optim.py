@@ -19,6 +19,8 @@ backward and the next forward.
 """
 from __future__ import annotations
 
+import weakref
+
 import numpy as np
 import torch
 import torch.nn as nn
@@ -26,7 +28,10 @@ from torch.optim import Optimizer
 
 from . import _lib
 
-flat_registry: dict = {}   # id(param) → FlatParams (lets DistributedDataParallel find the optimizer's layout)
+# id(param) → FlatParams (lets DistributedDataParallel find the optimizer's layout).  Weak: an entry lives as long as its
+# optimizer's flat buffers, which hold the parameters (so their ids are not reused); a strong dict kept every optimizer's
+# parameter, gradient, momentum and shadow buffers on the device for the life of the process.
+flat_registry: weakref.WeakValueDictionary = weakref.WeakValueDictionary()
 
 _ALIGN = 64  # elements; keeps every tensor view 256-byte aligned and every segment float4-aligned
 

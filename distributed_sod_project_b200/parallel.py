@@ -36,8 +36,8 @@ class DistributedDataParallel(nn.Module):
         params = [p for p in module.parameters() if p.requires_grad]
         if optimizer is not None:
             self.flat = optimizer.flat
-        elif params and id(params[0]) in _flat_registry:
-            self.flat = _flat_registry[id(params[0])]
+        elif params:
+            self.flat = _flat_registry.get(id(params[0]))
         if self.world == 1:
             return
         if self.flat is None:

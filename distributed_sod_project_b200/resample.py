@@ -1,7 +1,9 @@
-"""Channels-last ×2 bilinear up-sampling (+ fused add) and 2×2 average pooling, backed by csrc/resample.cu.
+"""Channels-last ×2 bilinear up-sampling (+ fused add), 2×2 average pooling and nearest ×2 up-sampling, backed by
+csrc/resample.cu and csrc/nearest.cu.
 
-These are the reference's `cus_sample` / `upsample_add` (utils/tensor_ops.py:12-25) and `h2l_pool`
-(module/MyLightModule.py:14).  The model plugins call `upsample2x` / `upsample2x_add` / `avgpool2x2` through
+These are the reference's `cus_sample` / `upsample_add` (utils/tensor_ops.py:12-25), `h2l_pool`
+(module/MyLightModule.py:14) and LightAIM's `nn.Upsample(scale_factor=2, mode="nearest")` (module/MyLightModule.py:64,146).
+The model plugins call `upsample2x` / `upsample2x_add` / `avgpool2x2` / `upsample2x_nearest` through
 `network/blocks.py`; anything the kernels do not cover (CPU tensors, a ratio other than exactly 2, C % 8 != 0)
 returns None so the caller keeps the torch op — those are shapes the TestModel never produces on the hot path.
 """
@@ -100,6 +102,37 @@ def avgpool2x2(x: torch.Tensor) -> torch.Tensor | None:
     if not _ok(x) or x.shape[2] % 2 or x.shape[3] % 2:
         return None
     return _AvgPool2x2.apply(x)
+
+
+class _UpNearest2x(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x):
+        x = _rows(x)
+        n, c, h, w = x.shape
+        y = torch.empty((n, c, 2 * h, 2 * w), dtype=x.dtype, device=x.device, memory_format=torch.channels_last)
+        rc = _lib.lib().sod_upsample2x_nearest_fwd(x.data_ptr(), y.data_ptr(), n, h, w, c, _lib.dtype_code(x.dtype), _lib.stream_ptr())
+        _lib.check(rc, "sod_upsample2x_nearest_fwd")
+        _lib.count_launch()
+        ctx.shape = (n, c, h, w)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        n, c, h, w = ctx.shape
+        dy = _rows(dy)
+        dx = torch.empty((n, c, h, w), dtype=dy.dtype, device=dy.device, memory_format=torch.channels_last)
+        rc = _lib.lib().sod_upsample2x_nearest_bwd(dy.data_ptr(), dx.data_ptr(), n, h, w, c, _lib.dtype_code(dy.dtype), _lib.stream_ptr())
+        _lib.check(rc, "sod_upsample2x_nearest_bwd")
+        _lib.count_launch()
+        return dx
+
+
+def upsample2x_nearest(x: torch.Tensor) -> torch.Tensor | None:
+    """`nn.Upsample(scale_factor=2, mode="nearest")` of the LightAIM neck, in x's dtype; None where the kernels do not
+    cover x (caller falls back to F.interpolate)"""
+    if not _ok(x):
+        return None
+    return _UpNearest2x.apply(x)
 
 
 class _MaxPool3x3s2(torch.autograd.Function):

@@ -145,13 +145,14 @@ class _SyncBNFn(torch.autograd.Function):
         direct = (wg is not None and bg is not None and wg.dtype == torch.float32 and bg.dtype == torch.float32
                   and wg.is_contiguous() and bg.is_contiguous() and ctx.weight_ref.requires_grad and ctx.bias_ref.requires_grad)
         # folded conv biases: the kernel adds Σ_rows dz into a bound .grad (FusedSGD's bf16/fp32 flat buffers) when there
-        # is one, else into a zeroed temporary that is handed to autograd
+        # is one, else into a zeroed temporary that is handed to autograd (always for a non-leaf bias, such as the sum of
+        # two biases that `blocks.conv3_bn_act` folds into one slot: autograd routes it on)
         cb1, cb2 = ctx.cb
         dcb, ret_cb = [None, None], [None, None]
         for i, cb in enumerate((cb1, cb2)):
             if cb is None or not cb.requires_grad:
                 continue
-            gbound = getattr(cb, "grad", None)
+            gbound = cb.grad if cb.is_leaf else None
             if gbound is not None and gbound.dtype == cb.dtype and gbound.is_contiguous():
                 dcb[i] = gbound
             else:

@@ -303,11 +303,17 @@ int sod_syncbn_bwd(const void* dy, const void* x, const void* pre_add, const voi
  *   `add` (may be NULL) is the tensor `upsample_add` sums with, already at the output size.  (h, w) = INPUT size.
  *   The backward is a gather (no atomics): deterministic.
  * sod_avgpool2x2_*: AvgPool2d((2,2), stride=2) — `h2l_pool` (module/MyLightModule.py:14); (h_out, w_out) = OUTPUT size.
+ * sod_upsample2x_nearest_*: nn.Upsample(scale_factor=2, mode="nearest") — LightAIM's `l2h_up` / `upsample`
+ *   (module/MyLightModule.py:64,146); (h, w) = INPUT size, any h, w ≥ 1.  The forward copies 16-byte packets (bit-exact);
+ *   the backward sums the four dy of each input pixel in row-major order from 0 in fp32 and rounds once (gather, no
+ *   atomics: deterministic).
  * ------------------------------------------------------------------------------------------------ */
 int sod_upsample2x_bilinear_fwd(const void* x, const void* add, void* y, int n, int h, int w, int c, int dtype, void* stream);
 int sod_upsample2x_bilinear_bwd(const void* dy, void* dx, int n, int h, int w, int c, int dtype, void* stream);
 int sod_avgpool2x2_fwd(const void* x, void* y, int n, int h_out, int w_out, int c, int dtype, void* stream);
 int sod_avgpool2x2_bwd(const void* dy, void* dx, int n, int h_out, int w_out, int c, int dtype, void* stream);
+int sod_upsample2x_nearest_fwd(const void* x, void* y, int n, int h, int w, int c, int dtype, void* stream);
+int sod_upsample2x_nearest_bwd(const void* dy, void* dx, int n, int h, int w, int c, int dtype, void* stream);
 
 /* Column sum of a channels-last matrix [rows, c] (c a power-of-two multiple of 8, ≤ 2048) into out[c] (same dtype, fp32
  * accumulation, deterministic): the bias gradient Σ_rows dy of a convolution that does not feed a BatchNorm — the five

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Generate the golden vectors of one backbone plugin by running the UNMODIFIED reference on CPU.
 
-    SOD_REFERENCE=/path/to/Distributed-SOD-Project python tools/make_golden_backbones.py {vgg16|wsgn_res50|wsgn_resnext50}
+    SOD_REFERENCE=/path/to/Distributed-SOD-Project python tools/make_golden_backbones.py {vgg16|wsgn_res50|wsgn_resnext50|aim_res50}
 
 Writes tests/golden/model_<backbone>_init.npz, the fp32 trajectories step_<backbone>_w1_s64 / _w1_s128 / _w2_s64 and
 the float64 runs of their first two iterations (`_fp64`).  W=2 is the concatenated-batch construction of
@@ -144,8 +144,86 @@ def install_wsgn_resnext_backbone():
     return "res50"
 
 
+def _aim_probe_params(model):
+    """small fixed probes of the post-step parameters (`trans32` does not exist in this model)"""
+    sd = dict(model.named_parameters())
+    keys = ["div_2.0.weight", "div_4.1.0.conv1.weight", "div_32.2.bn3.weight", "div_32.2.conv3.weight",
+            "trans.conv0.h2h_0.weight", "trans.conv2.bnm_1.bias", "trans.conv4.identity.bias", "sim2.bnh_2.bias",
+            "upconv1.basicconv.0.weight", "classifier.weight", "classifier.bias"]
+    return {k: sd[k].detach().reshape(-1)[:64].numpy().copy() for k in keys}
+
+
+def install_aim_model():
+    """The reference ships MINet's `LightAIM` neck (module/MyLightModule.py:216-236) but no network on it.  MINet_Res50
+    puts it between the ResNet-50 and the SIM decoder, so the model is composed here, from the reference's own
+    `Backbone_ResNet50_in3`, `LightAIM`, `SIM`, `BasicConv2d`, `upsample_add` and `cus_sample`, in the order backbone,
+    trans (= LightAIM((64, 256, 512, 1024, 2048), (64,) * 5)), sim32 … sim2, upconv32 … upconv2, upconv1, classifier;
+    forward is the reference `res50`'s with `trans(...)` giving the five laterals.  It is registered as
+    `network.aim_res50`.  The neck keeps torch's default conv and BN init, as the reference's module does.
+
+    The reference's own fp32 distance from its float64 run, |loss| and max |logits| difference:
+
+        vector      iteration 0: loss, logits       iteration 1: loss, logits
+        w1_s64      9.8e-07, 9.5e-04                2.2e-04, —
+        w1_s128     1.4e-07, 2.9e-04                1.8e-05, 1.2e-01
+        w2_s64      9.7e-07, 2.1e-04 (worst rank)   5.6e-04, — (worst rank)
+
+    The 64² iteration-0 logits are already 6.7e-4 of their largest magnitude (1.42) from the float64 run, so the
+    trajectory test allows the reference's noise from iteration 0 on.  One SGD step amplifies the 128² logits' fp32
+    rounding to 1.2e-1 (7 % of their largest magnitude, 1.63): the neck's 91 M parameters take the same step size."""
+    mg.install_reference()
+    import network
+    from backbone.origin.from_origin import Backbone_ResNet50_in3
+    from module.BaseBlocks import BasicConv2d
+    from module.MyLightModule import SIM, LightAIM
+    from utils.tensor_ops import cus_sample, upsample_add
+
+    class aim_res50(nn.Module):
+        def __init__(self):
+            super().__init__()
+            self.upsample_add = upsample_add
+            self.upsample = cus_sample
+            self.div_2, self.div_4, self.div_8, self.div_16, self.div_32 = Backbone_ResNet50_in3()
+            self.trans = LightAIM(iC_list=(64, 256, 512, 1024, 2048), oC_list=(64, 64, 64, 64, 64))
+            self.sim32 = SIM(64, 32)
+            self.sim16 = SIM(64, 32)
+            self.sim8 = SIM(64, 32)
+            self.sim4 = SIM(64, 32)
+            self.sim2 = SIM(64, 32)
+            self.upconv32 = BasicConv2d(64, 64, kernel_size=3, stride=1, padding=1)
+            self.upconv16 = BasicConv2d(64, 64, kernel_size=3, stride=1, padding=1)
+            self.upconv8 = BasicConv2d(64, 64, kernel_size=3, stride=1, padding=1)
+            self.upconv4 = BasicConv2d(64, 64, kernel_size=3, stride=1, padding=1)
+            self.upconv2 = BasicConv2d(64, 32, kernel_size=3, stride=1, padding=1)
+            self.upconv1 = BasicConv2d(32, 32, kernel_size=3, stride=1, padding=1)
+            self.classifier = nn.Conv2d(32, 1, 1)
+
+        def forward(self, in_data):
+            in_data_2 = self.div_2(in_data)
+            in_data_4 = self.div_4(in_data_2)
+            in_data_8 = self.div_8(in_data_4)
+            in_data_16 = self.div_16(in_data_8)
+            in_data_32 = self.div_32(in_data_16)
+            in_data_2, in_data_4, in_data_8, in_data_16, in_data_32 = self.trans(
+                in_data_2, in_data_4, in_data_8, in_data_16, in_data_32)
+            out_data_32 = self.upconv32(self.sim32(in_data_32) + in_data_32)
+            out_data_16 = self.upsample_add(out_data_32, in_data_16)
+            out_data_16 = self.upconv16(self.sim16(out_data_16) + out_data_16)
+            out_data_8 = self.upsample_add(out_data_16, in_data_8)
+            out_data_8 = self.upconv8(self.sim8(out_data_8) + out_data_8)
+            out_data_4 = self.upsample_add(out_data_8, in_data_4)
+            out_data_4 = self.upconv4(self.sim4(out_data_4) + out_data_4)
+            out_data_2 = self.upsample_add(out_data_4, in_data_2)
+            out_data_2 = self.upconv2(self.sim2(out_data_2) + out_data_2)
+            return self.classifier(self.upconv1(self.upsample(out_data_2, scale_factor=2)))
+
+    network.aim_res50 = aim_res50
+    mg._probe_params = _aim_probe_params
+    return "aim_res50"
+
+
 INSTALLERS = {"vgg16": install_vgg_model, "wsgn_res50": install_wsgn_backbone,
-              "wsgn_resnext50": install_wsgn_resnext_backbone}
+              "wsgn_resnext50": install_wsgn_resnext_backbone, "aim_res50": install_aim_model}
 
 
 def main():
