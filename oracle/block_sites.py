@@ -1,5 +1,5 @@
-"""Block "sites" of the four TestModel backbones (`res50`, `vgg16`, `wsgn_res50`, `wsgn_resnext50`): each model cut into
-the pieces `_TestModel.forward` strings together, so that each can be run and differentiated on its own
+"""Block "sites" of the five TestModel models (`res50`, `vgg16`, `wsgn_res50`, `wsgn_resnext50`, `aim_res50`): each model
+cut into the pieces `_TestModel.forward` strings together, so that each can be run and differentiated on its own
 (tests/test_block_sites_cpu.py, tests/test_gpu_block_seams.py).  Every function takes the model's name, `res50` by
 default.
 
@@ -16,6 +16,9 @@ sees.
   GroupNorm(32) and their convolutions weight-standardised, their decoder is `res50`'s.
 * `vgg16`'s backbone sites are its five slices `div_2` … `div_32`, at strides 1 … 16; `div_4` … `div_32` open with a 2×2
   max-pool.  Its decoder sites carry `res50`'s names at half `res50`'s stride, and its head has no ×2 up-sample.
+* `aim_res50` has `res50`'s backbone, SIM, upconv, upsample_add and head sites; its five `trans*` convolutions are
+  replaced by the LightAIM neck's blocks `trans.conv0` … `trans.conv4` (`NECK_TAPS`), each taking two or three
+  backbone taps (post-ReLU, so drawn non-negative: `relu_inputs`).  A neck site's `stride` is that of its output.
 """
 from __future__ import annotations
 
@@ -30,7 +33,9 @@ TAPS = (32, 16, 8, 4, 2)
 TAP_CHANNELS = {32: 2048, 16: 1024, 8: 512, 4: 256, 2: 64}
 STAGES = ((4, 64, 3), (8, 128, 4), (16, 256, 6), (32, 512, 3))     # (stride, width, units) of ResNet-50
 SIZES = (256, 288, 320, 352, 384)                                  # 288 / 352: odd 9×9 / 11×11 stride-32 map
-MODELS = ("res50", "vgg16", "wsgn_res50", "wsgn_resnext50")
+MODELS = ("res50", "vgg16", "wsgn_res50", "wsgn_resnext50")     # the backbones, each with every decoder site
+NECK_MODELS = ("aim_res50",)                                      # res50 with the LightAIM neck in place of trans*
+ALL_MODELS = MODELS + NECK_MODELS                                 # every model with a site table
 WSGN = ("wsgn_res50", "wsgn_resnext50")
 VGG_TAP_CHANNELS = {32: 512, 16: 512, 8: 256, 4: 128, 2: 64}       # `vgg16.tap_channels`
 VGG_SLICE_IN = {2: 3, 4: 64, 8: 128, 16: 256, 32: 512}             # input channels of slice div_s, at stride s // 4 (div_2: 1)
@@ -38,7 +43,13 @@ VGG_SLICE_IN = {2: 3, 4: 64, 8: 128, 16: 256, 32: 512}             # input chann
 BN, UP, AVG, MAX, CONVB, LOSS = ("_SyncBNFnBackward", "_Up2xBackward", "_AvgPool2x2Backward", "_MaxPool3x3s2Backward",
                                  "_ConvBiasBackward", "_FusedLossFnBackward")
 GN, WS, WSG, MAX2 = "_GroupNormFnBackward", "_WSFnBackward", "_WSGroupConvFnBackward", "_MaxPool2x2s2Backward"
-SEAM_NODES = (BN, UP, AVG, MAX, CONVB, GN, WS, WSG, MAX2)
+NEAR = "_UpNearest2xBackward"
+SEAM_NODES = (BN, UP, AVG, MAX, CONVB, GN, WS, WSG, MAX2, NEAR)
+# LightAIM: block i of `trans` → (the backbone strides it takes, in argument order; the stride of its output)
+NECK_TAPS = {0: ((2, 4), 2), 1: ((2, 4, 8), 4), 2: ((4, 8, 16), 8), 3: ((8, 16, 32), 16), 4: ((16, 32), 32)}
+# per block: (BatchNorms, nearest ×2 up-samples, 2×2 average pools) of its forward — Conv2nV1 (blocks 0 and 4, main
+# stream 0 / 1) and Conv3nV1 (blocks 1 … 3)
+NECK_NODES = {0: (6, 2, 1), 1: (8, 3, 3), 2: (8, 3, 3), 3: (8, 3, 3), 4: (6, 1, 2)}
 
 
 @dataclass(frozen=True)
@@ -52,6 +63,7 @@ class Site:
     representative: bool = True               # GPU grid (`grid`); the other plain bottlenecks repeat a tested one
     loss: bool = False                        # head: the fused BCE + CEL loss follows
     input_grad: tuple[bool, ...] = field(default=(True,))
+    relu_inputs: bool = False                 # the inputs are post-ReLU maps: draw them non-negative
 
 
 def _bottleneck_site(stride, unit, cin, width, down):
@@ -83,8 +95,8 @@ def _vgg_head_run(mods, d2):
 
 
 def _check(model_name):
-    if model_name not in MODELS:
-        raise ValueError(f"no site table for model {model_name!r}; one of {MODELS}")
+    if model_name not in ALL_MODELS:
+        raise ValueError(f"no site table for model {model_name!r}; one of {ALL_MODELS}")
 
 
 def _resnet_backbone() -> list[Site]:
@@ -109,11 +121,18 @@ def _vgg_backbone() -> list[Site]:
     return out
 
 
-def _decoder(tap_channels, half) -> list[Site]:
-    """trans* … head; `half`: every tap sits at half `res50`'s stride (vgg16)"""
+def _neck_site(i) -> Site:
+    path = f"trans.conv{i}"
+    taps, out = NECK_TAPS[i]
+    return Site(path, (path,), lambda S, b, taps=taps: [(b, TAP_CHANNELS[t], S // t, S // t) for t in taps],
+                lambda mods, *xs, p=path: mods[p](*xs), "neck", out, input_grad=(True,) * len(taps), relu_inputs=True)
+
+
+def _decoder(tap_channels, half, trans=True) -> list[Site]:
+    """trans* … head; `half`: every tap sits at half `res50`'s stride (vgg16); `trans`: with the five trans* sites"""
     st = {s: s // 2 if half else s for s in TAPS}
     out = []
-    for s in TAPS:
+    for s in TAPS if trans else ():
         out.append(Site(f"trans{s}", (f"trans{s}",), lambda S, b, s=s: [(b, tap_channels[s], S // st[s], S // st[s])],
                         lambda mods, x, s=s: mods[f"trans{s}"](x), "trans", st[s]))
     for s in TAPS:
@@ -136,12 +155,17 @@ def sites(model_name: str = "res50") -> list[Site]:
     _check(model_name)
     if model_name == "vgg16":
         return _vgg_backbone() + _decoder(VGG_TAP_CHANNELS, half=True)
+    if model_name == "aim_res50":
+        return _resnet_backbone() + [_neck_site(i) for i in NECK_TAPS] + _decoder(TAP_CHANNELS, half=False, trans=False)
     return _resnet_backbone() + _decoder(TAP_CHANNELS, half=False)
 
 
 def grid(model_name: str = "res50") -> list[Site]:
     """the sites the GPU grid runs: the representative ones, without the WS-GN models' decoder (`res50`'s code at
-    `res50`'s shapes, which the `res50` rows already run)"""
+    `res50`'s shapes, which the `res50` rows already run); for `aim_res50` its five neck sites alone (the rest is
+    `res50`'s code at `res50`'s shapes)"""
+    if model_name == "aim_res50":
+        return [s for s in sites(model_name) if s.kind == "neck"]
     decoder = ("trans", "sim", "upconv", "upadd", "head")
     return [s for s in sites(model_name) if s.representative and not (model_name in WSGN and s.kind in decoder)]
 
@@ -170,8 +194,19 @@ def _grouped_conv_on_kernels(site: Site) -> bool:
 
 
 def dispatch(site: Site, size: int, amp: bool, model_name: str = "res50") -> dict[str, bool]:
-    """backward node → present, for the engine's forward of `site` at image size `size` (amp: 16-bit shadow weights)"""
+    """backward node → present, for the engine's forward of `site` at image size `size` (amp: 16-bit shadow weights).
+
+    The LightAIM neck sites (`aim_res50`) take every map at strides 2 … 16 through their 2×2 average pools; at every
+    size of SIZES (multiples of 32) those maps are even — only the stride-32 map is odd, 9² at 288² and 11² at 352², and
+    no neck block pools it — so every neck pool runs on the kernel.  Their nearest ×2 up-samples take any H, W and C % 8
+    == 0 (64 channels, 1024 in block 4).  Under amp the 1×1 `identity` convolution, called as a module, takes
+    `conv_bias` (C = 64); the 3×3 ones fold their biases into the SyncBN kernel.  `counts` gives the numbers."""
     _check(model_name)
+    if site.kind == "neck":
+        want = dict.fromkeys(SEAM_NODES, False)
+        want[BN] = want[NEAR] = want[AVG] = True
+        want[CONVB] = amp
+        return want
     hw = size // site.stride
     want = dict.fromkeys(SEAM_NODES, False)
     backbone = site.kind in ("stem", "pool", "down", "plain", "vpool")
@@ -192,6 +227,14 @@ def dispatch(site: Site, size: int, amp: bool, model_name: str = "res50") -> dic
     if site.kind == "trans":
         want[CONVB] = amp            # C = 64: sod_colsum's bias gradient, reached through the shadow-weight forward
     return want                      # head: the classifier's C = 1 never takes `conv_bias`
+
+
+def counts(site: Site, amp: bool) -> dict[str, int]:
+    """backward node → how many the engine's forward of the neck site `site` creates (`dispatch` says which)"""
+    if site.kind != "neck":
+        raise ValueError(f"{site.name}: node counts are kept for the neck sites only")
+    n_bn, n_near, n_avg = NECK_NODES[int(site.name[len("trans.conv"):])]
+    return {BN: n_bn, NEAR: n_near, AVG: n_avg, CONVB: 1 if amp else 0}
 
 
 def stock_twin(site: Site, model: nn.Module | None = None, dtype: torch.dtype = torch.float64,
@@ -258,7 +301,10 @@ def compose(model: nn.Module, image: torch.Tensor, model_name: str = "res50") ->
             for u in range(units):
                 x = run(f"div_{stride}.{u}", x)
             feats[stride] = x
-    lat = {s: run(f"trans{s}", feats[s]) for s in (2, 4, 8, 16, 32)}
+    if model_name == "aim_res50":
+        lat = {out: run(f"trans.conv{i}", *(feats[t] for t in taps)) for i, (taps, out) in NECK_TAPS.items()}
+    else:
+        lat = {s: run(f"trans{s}", feats[s]) for s in (2, 4, 8, 16, 32)}
     d = None
     for s in TAPS:
         x = lat[s] if d is None else run(f"upsample_add{s}", d, lat[s])

@@ -1,10 +1,12 @@
-"""ORACLE (test infrastructure only): the launch geometry of the resampling kernels, restated from csrc/resample.cu and
-csrc/maxpool.cu.
+"""ORACLE (test infrastructure only): the launch geometry of the resampling kernels, restated from csrc/resample.cu,
+csrc/maxpool.cu and csrc/nearest.cu.
 
-* The six grid-stride kernels (bilinear ×2, 2×2 average pool and 3×3/2 max pool, forward and backward) run `grid_for`
-  CTAs of 256 threads, at most 16 per SM, and thread t handles the 16-byte channel packets t, t + T, t + 2T, … of the
-  tensor it writes (T = grid·256).  The forward of the up-sample and the backward of the average pool write the larger
-  tensor, the other four the smaller one, so the packet count P of a shape differs by kernel.  `classify` puts P in a
+* The eight grid-stride kernels (bilinear ×2, 2×2 average pool, 3×3/2 max pool and nearest ×2, forward and backward) run
+  `grid_for` CTAs of 256 threads, at most 16 per SM, and thread t handles the 16-byte channel packets t, t + T, t + 2T, …
+  of the tensor it writes (T = grid·256).  The forward of the bilinear up-sample and the backward of the average pool
+  write the larger tensor, the max pool's two kernels and the other two the smaller one; the nearest kernels run one
+  thread per packet of the smaller (input) side in both directions, the forward writing its four copies, the backward
+  gathering its four taps.  So the packet count P of a shape differs by kernel.  `classify` puts P in a
   wave regime: a partial wave below the cap, exactly one full pass, one full pass plus a ragged one, two or more passes
   ragged or exact.
 * `sod_colsum` runs min(⌈rows/8R⌉, 2·#SMs, 296) CTAs of 256 threads, L = C/8 lanes by R = 256/L rows.  Thread (b, r0)
@@ -20,7 +22,7 @@ from dataclasses import dataclass
 
 import numpy as np
 
-K_THREADS = 256            # resample.cu and maxpool.cu kThreads
+K_THREADS = 256            # resample.cu, maxpool.cu and nearest.cu kThreads
 K_CTAS_PER_SM = 16         # grid_for's cap: 16·#SMs CTAs
 COLSUM_THREADS = 256
 COLSUM_PASSES = 8          # at least eight row passes per CTA before the grid grows
@@ -29,25 +31,28 @@ COLSUM_MAX_GRID = 296
 COLSUM_MAX_C = 2048
 COLSUM_UNROLL = 4
 
-KERNELS = ("upsample_fwd", "upsample_bwd", "avgpool_fwd", "avgpool_bwd", "maxpool_fwd", "maxpool_bwd")
+KERNELS = ("upsample_fwd", "upsample_bwd", "avgpool_fwd", "avgpool_bwd", "maxpool_fwd", "maxpool_bwd")   # what res50 runs
+NEAREST_KERNELS = ("nearest_fwd", "nearest_bwd")                  # the LightAIM neck's (aim_res50)
+GRID_STRIDE_KERNELS = KERNELS + NEAREST_KERNELS                   # all eight
 DTYPES = ("float32", "bfloat16", "float16")
 WAVES = ("partial", "1", "1+ragged", ">=2 ragged", ">=2 exact")
 LANES = tuple(1 << k for k in range(9))                   # L = C/8 = 1 … 256
 COLSUM_AXES = dict(L=LANES, grid=("below", "cap"), tail=(0, 1, 2, 3), idle=("yes",), rows=("1",))
 
 
-# ---- the six grid-stride kernels ---------------------------------------------------------------------------------
+# ---- the eight grid-stride kernels -------------------------------------------------------------------------------
 def grid_for(packets, sm_count):
     return int(min(max(-(-packets // K_THREADS), 1), K_CTAS_PER_SM * sm_count))
 
 
 def packets(kernel, shape):
-    """16-byte packets the kernel writes for the forward input `shape` = (n, c, h, w); the avg-pool needs even h, w"""
+    """16-byte packets the kernel's loop runs over for the forward input `shape` = (n, c, h, w) (the nearest kernels: one
+    per input packet in both directions); the avg-pool needs even h, w"""
     n, c, h, w = shape
     c8 = c // 8
     if kernel == "upsample_fwd":
         return n * 2 * h * 2 * w * c8
-    if kernel in ("upsample_bwd", "maxpool_bwd", "avgpool_bwd"):
+    if kernel in ("upsample_bwd", "maxpool_bwd", "avgpool_bwd", "nearest_fwd", "nearest_bwd"):
         return n * h * w * c8
     if kernel == "avgpool_fwd":
         return n * (h // 2) * (w // 2) * c8
@@ -81,7 +86,8 @@ def classify(p, sm_count):
 
 
 def _multiple(kernel):
-    """P is a multiple of 4 where the kernel writes the ×2 side of the op"""
+    """P is a multiple of 4 where the kernel writes the ×2 side of the op (not the nearest kernels: one thread per input
+    packet)"""
     return 4 if kernel in ("upsample_fwd", "avgpool_bwd") else 1
 
 

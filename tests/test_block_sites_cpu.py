@@ -1,12 +1,12 @@
-"""The block-site tables of oracle/block_sites.py against the models they cut up (CPU only), for each of the four
-backbones (`res50`, `vgg16`, `wsgn_res50`, `wsgn_resnext50`):
+"""The block-site tables of oracle/block_sites.py against the models they cut up (CPU only), for each of the five
+models (`res50`, `vgg16`, `wsgn_res50`, `wsgn_resnext50`, `aim_res50`):
 
 * every parameter and buffer of the model belongs to exactly one site;
 * the sites, run one after the other, are the model's forward bit for bit (fp32, stock modules) and leave the same
   norm buffers behind;
 * the site shapes are what the model feeds its modules;
-* `dispatch` — which of the engine's resampling / max-pool / column-sum / GroupNorm / weight-standardisation kernels each
-  site reaches — agrees with the predicates of `resample.py`, `wsgn.py` and `network/blocks.py` at 256², 288², 320², 352²
+* `dispatch` — which of the engine's resampling / max-pool / nearest / column-sum / GroupNorm / weight-standardisation
+  kernels each site reaches (and, for the LightAIM neck sites, `counts`: how often) — agrees with the predicates of `resample.py`, `wsgn.py` and `network/blocks.py` at 256², 288², 320², 352²
   and 384².  The forward runs on CPU tensors that report `is_cuda`, through the engine's own GroupNorm and WS modules
   (`convert_wsgn_model`), with the kernels' autograd Functions (and `wsgn.standardize_weight`, whose `is_cuda` check
   reads the CPU weight) replaced by recorders that hand back the torch result, so the predicates are evaluated exactly
@@ -23,12 +23,13 @@ import torch.nn.functional as F
 from oracle import block_sites as bs
 
 
-MODELS = list(bs.MODELS)
+MODELS = list(bs.ALL_MODELS)
 PLUGINS = [m for m in MODELS if m != "res50"]      # res50's checks keep their own (older) test names
 RESNET_BACKBONE = ["stem", "pool+div_4.1.0", "div_4.1.1", "div_8.0", "div_8.1", "div_16.0", "div_16.1", "div_32.0",
                    "div_32.1"]
 DECODER = [f"{k}{s}" for k in ("trans", "sim", "upconv") for s in bs.TAPS] + [f"upsample_add{s}" for s in bs.TAPS[1:]] + \
     ["head"]
+NECK = [f"trans.conv{i}" for i in range(5)]
 
 
 def _model(name="res50"):
@@ -52,6 +53,10 @@ def _ownership(name):
         bs.modules(model, s)
     rep = [s.name for s in table if s.representative]
     backbone = [f"div_{s}" for s in reversed(bs.TAPS)] if name == "vgg16" else RESNET_BACKBONE
+    if name == "aim_res50":                          # the neck in place of trans*; the grid runs the neck alone
+        assert rep == backbone + NECK + [d for d in DECODER if not d.startswith("trans")]
+        assert [s.name for s in bs.grid(name)] == NECK
+        return
     assert rep == backbone + DECODER
     assert [s.name for s in bs.grid(name)] == (backbone if name in bs.WSGN else rep)
 
@@ -96,7 +101,7 @@ def _shapes(name):
 
     def hook(name):
         def fn(mod, args):
-            seen.setdefault(name, tuple(args[0].shape))
+            seen.setdefault(name, [tuple(a.shape) for a in args])
         return fn
 
     for s in bs.sites(name):
@@ -104,7 +109,7 @@ def _shapes(name):
             model.get_submodule(s.paths[0]).register_forward_pre_hook(hook(s.name))
     model.get_submodule("upconv1").register_forward_pre_hook(hook("upconv1"))
     def head_input(mod, args, out):                   # the head's input d2 is upconv2's output
-        seen.setdefault("head", tuple(out.shape))
+        seen.setdefault("head", [tuple(out.shape)])
 
     model.get_submodule("upconv2").register_forward_hook(head_input)
     with torch.no_grad():
@@ -112,9 +117,9 @@ def _shapes(name):
     assert len(seen) == len([s for s in bs.sites(name) if s.paths]) + 1, sorted(seen)
     for site, shape in seen.items():
         if site == "upconv1":
-            assert shape == (1, 32, 128, 128)                # res50 up-samples d2 ×2 first, vgg16 does not
+            assert shape == [(1, 32, 128, 128)]              # res50 up-samples d2 ×2 first, vgg16 does not
         else:
-            assert shape == tuple(table[site].shapes(128, 1)[0]), site
+            assert shape == [tuple(sh) for sh in table[site].shapes(128, 1)], site
 
 
 def test_site_shapes_are_what_the_model_feeds_them():
@@ -155,6 +160,7 @@ def _recording():
         (resample, "_MaxPool3x3s2"): lambda x: F.max_pool2d(x, 3, 2, 1),
         (resample, "_MaxPool2x2s2"): lambda x: F.max_pool2d(x, 2, 2),
         (resample, "_ConvBias"): lambda x, w, b, *conf: F.conv2d(x, w, b, *conf),
+        (resample, "_UpNearest2x"): lambda x: F.interpolate(x, scale_factor=2, mode="nearest"),
         (wsgn, "_GroupNormFn"): gn,
         (wsgn, "_WSGroupConvFn"): lambda x, w, dtype, eps, stride: F.conv2d(x, std(w), None, stride, 1, 1, 32),
     }
@@ -199,16 +205,22 @@ def test_dispatch_matches_the_engine_predicates(name, size):
             site.run(mods, *xs)
         want = bs.dispatch(site, size, False, name)
         got = set(taken)
-        for node in (bs.UP, bs.AVG, bs.MAX, bs.MAX2, bs.GN, bs.WS, bs.WSG):
+        for node in (bs.UP, bs.AVG, bs.MAX, bs.MAX2, bs.GN, bs.WS, bs.WSG, bs.NEAR):
             assert (node in got) == want[node], (name, site.name, size, node, taken)
         assert bs.CONVB not in got                       # plain convolutions never take conv_bias
+        if site.kind == "neck":                          # stock BatchNorms here: the SyncBN count is the GPU walk's
+            for node in (bs.NEAR, bs.AVG):
+                assert taken.count(node) == bs.counts(site, False)[node], (site.name, size, node, taken)
         if site.kind == "sim":
             assert want[bs.UP] == want[bs.AVG] == (name == "vgg16" or not odd or site.stride != 32)
-        # under amp the shadow-weight forward offers every biased convolution called as a module to `conv_bias`
+        # under amp the shadow-weight forward offers every biased convolution called as a module to `conv_bias`: all of
+        # those of trans* and the head, the neck's 1×1 `identity` alone (its 3×3 ones fold their biases into the SyncBN
+        # kernel)
         with _recording() as taken, torch.no_grad(), torch.enable_grad():
             for p, m in mods.items():
-                for _, conv in m.named_modules():
-                    if isinstance(conv, torch.nn.Conv2d) and conv.bias is not None and site.kind in ("trans", "head"):
+                for cname, conv in m.named_modules():
+                    as_module = site.kind in ("trans", "head") or (site.kind == "neck" and cname == "identity")
+                    if isinstance(conv, torch.nn.Conv2d) and conv.bias is not None and as_module:
                         w = conv.weight.detach().to(torch.bfloat16).as_subclass(_Cudaish)
                         x = torch.zeros(1, conv.in_channels, 4, 4, dtype=torch.bfloat16).as_subclass(_Cudaish)
                         resample.conv_bias(conv, x, w, conv.bias.detach().to(torch.bfloat16).as_subclass(_Cudaish))

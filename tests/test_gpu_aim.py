@@ -1,9 +1,9 @@
 """`aim_res50` / `cp_aim_res50` (ResNet-50, MINet's LightAIM neck, the TestModel decoder) on the engine: the reference's
-fp32 trajectories, graph replay and activation checkpointing bit for bit, every parameter gradient against float64, each
-neck block alone through the engine's seams, the fp16 loss scaler on a neck overflow, the command line, and two ranks."""
+fp32 trajectories, graph replay and activation checkpointing bit for bit, every parameter gradient against float64, the
+backward nodes of a whole forward, the fp16 loss scaler on a neck overflow, the command line, and two ranks.  Each neck
+block alone, run through the real Trainer's seams against float64, is a row of tests/test_gpu_block_seams.py."""
 from __future__ import annotations
 
-import copy
 import socket
 import sys
 
@@ -93,67 +93,6 @@ def test_iteration_gradients_match_fp64(dtype, A):
     med = float(np.median(list(es.values())))
     worst = max((e(eng, n) / (es[n] + med), n) for n in ref)
     assert worst[0] <= A, f"{worst[1]}: engine error {worst[0]:.2f}x (stock + median)"
-
-
-# -- each neck block alone ---------------------------------------------------------------------------------------------
-_TAP = {2: 64, 4: 256, 8: 512, 16: 1024, 32: 2048}
-_BLOCK_TAPS = {0: (2, 4), 1: (2, 4, 8), 2: (4, 8, 16), 3: (8, 16, 32), 4: (16, 32)}
-_BLOCK_NODES = {0: (2, 1), 1: (3, 3), 2: (3, 3), 3: (3, 3), 4: (1, 2)}        # (nearest up-samples, average pools)
-_BLOCK_OUT = {0: 2, 1: 4, 2: 8, 3: 16, 4: 32}                                    # stride of each block's output
-
-
-def _block_run(block, taps, out, dtype, engine, size=128, n=2):
-    from distributed_sod_project_b200 import resample
-    from distributed_sod_project_b200.syncbn import convert_syncbn_model
-    g = torch.Generator().manual_seed(7)
-    xs = [torch.randn(n, _TAP[s], size // s, size // s, generator=g).relu() for s in taps]
-    dy = torch.randn(n, 64, size // out, size // out, generator=g)
-    if dtype == torch.float64:
-        mod, xs, dy = block.double().cuda(), [x.double().cuda() for x in xs], dy.double().cuda()
-    else:
-        mod = block.cuda().to(memory_format=torch.channels_last)
-        if engine:
-            mod = convert_syncbn_model(mod)
-        xs = [x.cuda().contiguous(memory_format=torch.channels_last) for x in xs]
-        dy = dy.cuda().to(dtype)
-    xs = [x.requires_grad_(True) for x in xs]
-    old = resample.ENABLED, blocks.INTERPOLATE_IN_ACTIVATION_DTYPE
-    resample.ENABLED = blocks.INTERPOLATE_IN_ACTIVATION_DTYPE = engine
-    try:
-        mod.train()
-        with torch.autocast("cuda", dtype=dtype, enabled=dtype in (torch.bfloat16, torch.float16)):
-            y = mod(*xs)
-        names = _node_names(y)
-        grads = torch.autograd.grad(y, [*xs, *mod.parameters()], dy.to(y.dtype))
-    finally:
-        resample.ENABLED, blocks.INTERPOLATE_IN_ACTIVATION_DTYPE = old
-    return [y.detach().double(), *(t.double() for t in grads)], names
-
-
-@pytest.mark.parametrize("dtype", DTYPES, ids=str)
-@pytest.mark.parametrize("i", range(5), ids=lambda i: f"conv{i}")
-def test_neck_block_through_the_seams_vs_fp64(i, dtype):
-    """trans.conv{i} alone, converted as the trainer converts it, against its float64 twin: output, input and parameter
-    gradients within 3× the stock torch block's error in the same precision (+ the median stock error); the backward
-    runs the SyncBN kernels for all its BatchNorms and the nearest / average-pool kernels for all its resamplings"""
-    from distributed_sod_project_b200 import network
-    from distributed_sod_project_b200.utils import init_seed
-    init_seed(0)
-    block = getattr(network.aim_res50().trans, f"conv{i}")
-    taps = _BLOCK_TAPS[i]
-    with _exact():
-        ref, _ = _block_run(copy.deepcopy(block), taps, _BLOCK_OUT[i], torch.float64, False)
-        stock, _ = _block_run(copy.deepcopy(block), taps, _BLOCK_OUT[i], dtype, False)
-        eng, names = _block_run(copy.deepcopy(block), taps, _BLOCK_OUT[i], dtype, True)
-    n_bn = sum(isinstance(m, torch.nn.BatchNorm2d) for m in block.modules())
-    assert names.count("_SyncBNFnBackward") == n_bn
-    assert (names.count("_UpNearest2xBackward"), names.count("_AvgPool2x2Backward")) == _BLOCK_NODES[i]
-    assert not [n for n in names if "Upsample" in n or "AvgPool2D" in n], sorted(set(names))
-    e = lambda g, k: float((g[k] - ref[k]).norm() / ref[k].norm().clamp_min(1e-300))  # noqa: E731
-    es = [e(stock, k) for k in range(len(ref))]
-    med = float(np.median(es))
-    worst = max((e(eng, k) / (es[k] + med), k) for k in range(len(ref)))
-    assert worst[0] <= 3.0, f"tensor {worst[1]}: engine error {worst[0]:.2f}x (stock + median)"
 
 
 @pytest.mark.parametrize("dtype", DTYPES, ids=str)

@@ -1,12 +1,15 @@
-"""Every block of `res50`, `vgg16`, `wsgn_res50` and `wsgn_resnext50` through the engine's autograd seam, against float64
-autograd of the same block.
+"""Every block of `res50`, `vgg16`, `wsgn_res50`, `wsgn_resnext50` and `aim_res50`'s LightAIM neck through the engine's
+autograd seam, against float64 autograd of the same block.
 
-`tests/test_gpu_model_grads.py` and `tests/test_gpu_backbones.py` check the seam (`_SyncBNFn`, `raw_backward`, `_Up2x`,
-`_AvgPool2x2`, `_MaxPool3x3s2`, `_MaxPool2x2s2`, `_ConvBias`, `_FusedLossFn`, `_GroupNormFn`, `_WSFn`, `_WSGroupConvFn`,
-the `network/blocks.py` helpers and the shadow-weight conv forward of `amp.py`) only through the whole model, which
-amplifies rounding about 10³-fold: in 16 bits a wiring fault hides there.  A single block has no such amplification, so
-here every site of oracle/block_sites.py is held close to float64 on its own.  Rows: every representative site of each
-backbone (`bs.grid`); the WS-GN models' decoder is `res50`'s code at `res50`'s shapes and runs in the `res50` rows.
+`tests/test_gpu_model_grads.py`, `tests/test_gpu_backbones.py` and `tests/test_gpu_aim.py` check the seam (`_SyncBNFn`,
+`raw_backward`, `_Up2x`, `_AvgPool2x2`, `_MaxPool3x3s2`, `_MaxPool2x2s2`, `_UpNearest2x`, `_ConvBias`, `_FusedLossFn`,
+`_GroupNormFn`, `_WSFn`, `_WSGroupConvFn`, the `network/blocks.py` helpers and the shadow-weight conv forward of `amp.py`)
+only through the whole model, which amplifies rounding about 10³-fold: in 16 bits a wiring fault hides there.  A single
+block has no such amplification, so here every site of oracle/block_sites.py is held close to float64 on its own.  Rows:
+every representative site of each backbone (`bs.grid`); the WS-GN models' decoder is `res50`'s code at `res50`'s shapes
+and runs in the `res50` rows, and so is everything of `aim_res50` but its five neck blocks `trans.conv0` … `trans.conv4`
+(their float64 twin: the stock BatchNorm, `F.interpolate(mode="nearest")` and `nn.AvgPool2d`; operands non-negative, as
+the backbone taps they stand for).
 
 * Engine: the real `Trainer` construction (`sgd_all`, SyncBN and WS-GN conversion, bf16 / fp16 `amp.initialize` with
   shadow weights and a real `FusedSGD`), one backbone's Trainers at a time.  Each site runs on the engine's own modules; the gradients are read where the step reads them —
@@ -34,7 +37,8 @@ decision moves one element of a norm layer's gradient by its full size (e2 ≈ 1
 for the stock yardstick as for the engine.  So when the A-rule fails, each is measured again against a float64 run that
 takes its own ReLU decisions, provided every decision where the engine differs from float64 sits within TIE_REL (the
 rounding of a 4608-term fp32 sum; four roundings of the 16-bit type) of zero.  Exact where an exact answer exists:
-the two folded biases of a `pre` BN get the same Σ dz, the `trans*` bias gradient under shadow weights is `colsum(dy)`,
+the two folded biases of a `pre` BN get the same Σ dz (and all three of a neck `conv3_bn_act`, whose second slot is the
+non-leaf `b2 + b3`), the `trans*` bias gradient under shadow weights is `colsum(dy)`,
 a residual's gradient is the ReLU-masked dy (for SyncBN and GroupNorm, in its own dtype), max-pool routes integer
 gradients as torch does, GroupNorm gives the same bits for NCHW and channels-last operands, the γ/β and WS weight
 gradients are the same bits added into a bound fp32 `.grad` or returned to autograd and a second backward doubles them,
@@ -63,16 +67,28 @@ The same measurements for the other rows (worst ratios without `upsample_add*`, 
                     fp16 0.96 (head, eval) / 1.56 (sim32)
     wsgn_res50      fp32 0.88 / 1.15 (div_4.1.1)   bf16 0.66 / 0.87 (bs 16 0.62 / 0.89)   fp16 0.65 / 0.94
     wsgn_resnext50  fp32 1.40 / 2.23 (div_4.1.1, eval)   bf16 0.62 / 0.90 (bs 16 0.67 / 0.89)   fp16 0.68 / 0.94
-Three cases took the ReLU-decision rule: wsgn_res50 div_16.0 fp32 eager (1 decision, |pre| / max 4.6e-8), vgg16 div_16
-fp32 eval (2, 2.1e-7) and vgg16 sim32 fp16 eval (7, 7.8e-5); each then holds at ratio ≤ 0.62 / 0.85.  Median stock e2
+Four cases took the ReLU-decision rule: wsgn_res50 div_16.0 fp32 eager (1 decision, |pre| / max 4.6e-8), vgg16 div_16
+fp32 eval (2, 2.1e-7), vgg16 sim32 fp16 eval (7, 7.8e-5) and aim_res50 trans.conv0 fp32 eval (3, 5.5e-8); each then holds
+at ratio ≤ 0.62 / 0.85 (aim_res50 0.92 / 1.50).  Median stock e2
 of the gradients (fp32 / bf16 / fp16; bf16 at 320² bs 16 within 10 % of 256² bs 2):
     vgg16  slices 8.8e-6-7.2e-3 / 5.2-9.1e-2 / 1.8-3.3e-2   sim* ≤ 9.6e-4 / 8.2-9.6e-2 / 2.5-3.1e-2
            trans* 2e-7 / 2.4e-3 / 3.0e-4   upconv* ≤ 4.6e-7 / 2.9-9.2e-3 / ≤ 3.6e-4   head 5.2e-7 / 1.6e-3 / 1.9e-4
     wsgn_res50 / wsgn_resnext50  stem 2.7e-7 / 3.1-3.2e-2 / 1.1e-2   bottlenecks ≤ 1.3e-3 / 4.9-7.8e-2 / 1.4-2.8e-2
 The bound stays above 0.25 for the 16-bit cases of the same kinds of site as in res50: bf16 (eager, eval and bs 16)
-WS-GN bottlenecks 0.31-0.56, VGG slices 0.25-0.51 and VGG SIM blocks 0.27-0.59.  With the new rows the file runs in
-about two and a half minutes.
+WS-GN bottlenecks 0.31-0.56, VGG slices 0.25-0.51 and VGG SIM blocks 0.27-0.59.
+    aim_res50 (neck)  fp32 e2 1.01 (conv2) emax 1.67 (conv0)   bf16 0.66 / 0.80 (bs 16 0.58 / 0.71)   fp16 0.71 / 1.14
+                      (conv4, eval)
+Median stock e2 of the neck blocks' gradients: fp32 1.8e-6-4.4e-6 (conv1 … conv4; conv0 1.3e-3, its C = 64 stride-2
+maps) / bf16 0.11-0.12 / fp16 0.040-0.049, eval 5.7e-7-6.3e-7 / 0.059-0.094 / 0.011-0.035.  As for the SIM blocks,
+whose structure the neck blocks share, the bf16 bound stays above 0.25 (0.37-0.79), and so does fp16 eager conv3 (0.28;
+the other fp16 cases 0.07-0.25): their wiring is held by the fp32 and eval cases, the exact checks and the dedicated
+`conv3_bn_act` cases below (the same bits of Σ dz for all three biases through a bound fp32 or 16-bit `.grad` or a
+temporary, in training and eval, with `b2` / `b3` frozen or one bias absent; a second backward doubles them; `zero_grad`
+clears a backward whose only writes went through the non-leaf slot; biases of two dtypes in the two slots are refused).
+In eval mode the folded biases' gradients are not zero in exact arithmetic and are measured against their own norm.
+The whole file runs in about two and a half minutes on an H100 80GB HBM3 at 700 W.
 """
+import collections
 import contextlib
 import statistics
 import types
@@ -110,7 +126,7 @@ def _row_id(model, name):
 
 
 # one row per (model, site) of the grid, grouped by model so that each backbone's Trainers are built once per test
-SITES = [pytest.param(m, s.name, id=_row_id(m, s.name)) for m in bs.MODELS for s in bs.grid(m)]
+SITES = [pytest.param(m, s.name, id=_row_id(m, s.name)) for m in bs.ALL_MODELS for s in bs.grid(m)]
 RESULTS: list = []               # (model/site, precision, path, worst e2 ratio, worst emax ratio, stock e2 median, max bound e2)
 
 
@@ -197,8 +213,8 @@ def _site_params(model, site):
 def _operands(site, dtype, size, batch, seed):
     """(inputs in the activation dtype, channels-last; upstream gradient maker; mask)"""
     g = torch.Generator(device="cuda").manual_seed(seed)
-    xs = [torch.randn(sh, device="cuda", generator=g).to(dtype).contiguous(memory_format=torch.channels_last)
-          for sh in site.shapes(size, batch)]
+    xs = [torch.randn(sh, device="cuda", generator=g) for sh in site.shapes(size, batch)]
+    xs = [(x.relu() if site.relu_inputs else x).to(dtype).contiguous(memory_format=torch.channels_last) for x in xs]
     mask = (torch.rand(batch, 1, size, size, device="cuda", generator=g) > 0.6).float() if site.loss else None
     dy_seed = seed + 7919
     return xs, mask, dy_seed
@@ -463,11 +479,11 @@ def _check_against_fp64(tr, stock_model, site, dtype, xs, mask, dy_seed, bufs0, 
         tag += " (own ReLU decisions)"
         w2, wm, med, mb = _yardstick(tag, _tensors(eng), _tensors(stk), _tensors(refs[1]), BOUND[dtype], slack,
                                      ref_eng=_tensors(refs[0]))
-    if site.kind == "sim":
-        # the SyncBN backward adds the same Σ dz into both folded biases of a conv_bn_act with `pre`
-        for a, b in (("h2h_1", "l2h_1"), ("l2l_1", "h2l_1"), ("h2h_2", "l2h_2")):
-            ga, gb = eng["grads"][f"{site.name}.{a}.bias"], eng["grads"][f"{site.name}.{b}.bias"]
-            assert torch.equal(ga, gb) and float(ga.abs().max()) > 0, f"{tag}: folded biases {a} / {b}"
+    # the SyncBN backward adds the same Σ dz into both folded biases of a conv_bn_act with `pre`, and conv3_bn_act's
+    # second slot (the sum of two biases) hands it on to both of them
+    for group in _folded(site):
+        gs = [eng["grads"][f"{site.name}.{a}.bias"] for a in group]
+        assert all(torch.equal(gs[0], g) for g in gs[1:]) and float(gs[0].abs().max()) > 0, f"{tag}: folded biases {group}"
     if site.loss:
         l64 = ref["loss"]
         assert abs(eng["loss"] - l64) <= BOUND[dtype][0] * abs(stk["loss"] - l64) + LOSS_SLACK[dtype] * abs(l64), \
@@ -475,6 +491,23 @@ def _check_against_fp64(tr, stock_model, site, dtype, xs, mask, dy_seed, bufs0, 
     RESULTS.append((row, NAME[dtype], path, w2, wm, med, mb))
     print(f"\n{tag}: worst ratio e2 {w2:.3f} emax {wm:.3f}; stock median gradient e2 {med:.2e}; largest e2 bound {mb:.2e}")
     return eng
+
+
+_SIM_FOLDED = (("h2h_1", "l2h_1"), ("l2l_1", "h2l_1"), ("h2h_2", "l2h_2"))
+# LightAIM: Conv2nV1 (blocks 0 and 4, merging into the high / low stream) and Conv3nV1 (blocks 1 … 3)
+_NECK_FOLDED = {0: (("h2h_1", "l2h_1"), ("l2l_1", "h2l_1"), ("h2h_2", "l2h_2")),
+                4: (("h2h_1", "l2h_1"), ("l2l_1", "h2l_1"), ("h2l_2", "l2l_2")),
+                **dict.fromkeys((1, 2, 3), (("h2h_1", "m2h_1"), ("h2m_1", "m2m_1", "l2m_1"), ("m2l_1", "l2l_1"),
+                                            ("h2m_2", "m2m_2", "l2m_2")))}
+
+
+def _folded(site):
+    """the groups of conv biases of the site that one BatchNorm's backward gives the same Σ dz"""
+    if site.kind == "sim":
+        return _SIM_FOLDED
+    if site.kind == "neck":
+        return _NECK_FOLDED[int(site.name[len("trans.conv"):])]
+    return ()
 
 
 def _restore(tr, site, bufs0):
@@ -647,19 +680,20 @@ def test_graph_replay_equals_eager(engines, model, name, dtype):
 
 
 def _walk(fn):
-    seen, stack, names = set(), [fn], set()
+    """backward node name → how many are reachable from fn"""
+    seen, stack, names = set(), [fn], collections.Counter()
     while stack:
         f = stack.pop()
         if f is None or f in seen:
             continue
         seen.add(f)
-        names.add(type(f).__name__)
+        names[type(f).__name__] += 1
         stack.extend(g for g, _ in f.next_functions)
     return names
 
 
 @pytest.mark.parametrize("size", bs.SIZES)
-@pytest.mark.parametrize("model,dtype", [pytest.param(m, d, id=_row_id(m, NAME[d])) for m in bs.MODELS for d in (_F32, _BF16)])
+@pytest.mark.parametrize("model,dtype", [pytest.param(m, d, id=_row_id(m, NAME[d])) for m in bs.ALL_MODELS for d in (_F32, _BF16)])
 def test_dispatch_matches_site_table(engines, model, size, dtype):
     tr = engines(model, dtype)
     for site in bs.grid(model):
@@ -675,6 +709,12 @@ def test_dispatch_matches_site_table(engines, model, size, dtype):
         for node, present in want.items():
             assert (node in names) == present, (model, site.name, size, NAME[dtype], node, sorted(names))
         assert (bs.LOSS in names) == site.loss
+        if site.kind == "neck":
+            # one SyncBN node per BatchNorm, every nearest up-sample and average pool on the kernels (none of torch's)
+            for node, k in bs.counts(site, dtype != _F32).items():
+                assert names[node] == k, (model, site.name, size, NAME[dtype], node, names[node], k)
+            assert names[bs.BN] == sum(isinstance(m, nn.BatchNorm2d) for m in tr.module.get_submodule(site.name).modules())
+            assert not [n for n in names if "Upsample" in n or "AvgPool2D" in n], sorted(names)
         _restore(tr, site, bufs0)
 
 
@@ -937,6 +977,199 @@ def test_zero_grad_clears_a_folded_bias_only_backward(dtype):
         assert torch.equal(bias_grad(), once), "stale folded-bias gradient survived zero_grad"
     finally:
         amp._cfg.update(enabled=False, dynamic=False, scale=1.0, good_steps=0, growth_interval=2000, owner=None, dev=None)
+
+
+# ---- seam cases on conv3_bn_act: three convolutions into one SyncBatchNorm --------------------------------------------
+_TRIPLE = ("h2m", "m2m", "l2m")
+_GRAD_PATHS = ("bound32", "temporary", "bound16")
+
+
+class _Triple(nn.Module):
+    """Conv3nV1's `bnm_1` / `bnm_2`: three 3×3 64→64 convolutions summed into one BatchNorm by `conv3_bn_act`, which
+    folds the first bias into the SyncBN kernel's first slot and `b2 + b3` (a non-leaf) into its second"""
+
+    def __init__(self, nobias=None):
+        super().__init__()
+        for name in _TRIPLE:
+            setattr(self, name, nn.Conv2d(64, 64, 3, 1, 1, bias=name != nobias))
+        self.bnm = nn.BatchNorm2d(64)
+
+    def forward(self, h, m, l):  # noqa: E741
+        from distributed_sod_project_b200.network.blocks import conv3_bn_act
+        return conv3_bn_act(self.h2m, self.bnm, h, (self.m2m, m), (self.l2m, l))
+
+
+def _triple(path, variant="all", frozen_affine=False):
+    """(model, optimizer | None, activation dtype): a `_Triple` converted as the Trainer converts it.  `path`: where the
+    bias gradients go — "bound32" (FusedSGD binds every .grad to its fp32 flat buffer), "bound16" (bf16 amp: the
+    biases are 16-bit shadows whose .grad is bound to the 16-bit flat buffer) or "temporary" (no optimizer: the kernel
+    adds into zeroed temporaries that autograd accumulates).  `variant`: "all", "<conv>_frozen" or "<conv>_nobias"."""
+    from distributed_sod_project_b200 import amp
+    from distributed_sod_project_b200.optim import make_optimizer
+    from distributed_sod_project_b200.syncbn import convert_syncbn_model
+    torch.manual_seed(40)
+    model = _Triple(nobias=variant[:3] if variant.endswith("_nobias") else None).cuda()
+    model = model.to(memory_format=torch.channels_last)
+    with torch.no_grad():
+        model.bnm.weight.uniform_(0.5, 1.5)
+        model.bnm.bias.normal_(0.0, 0.2)
+        model.bnm.running_mean.normal_(0.0, 0.3)
+        model.bnm.running_var.uniform_(0.5, 1.5)
+    if variant.endswith("_frozen"):
+        getattr(model, variant[:3]).bias.requires_grad_(False)
+    if frozen_affine:
+        model.bnm.requires_grad_(False)
+    opt = None if path == "temporary" else make_optimizer(model, "sgd_all", dict(lr=0.0, momentum=0.0, weight_decay=0.0))
+    model = convert_syncbn_model(model)
+    if path == "bound16":
+        model, opt = amp.initialize(model, opt, opt_level="O1", dtype=_BF16)
+        return model, opt, _BF16
+    return model, opt, _F32
+
+
+def _triple_inputs(dtype, seed):
+    """non-negative h, m, l (the neck's operands are post-ReLU maps) and dy, channels-last"""
+    return [_t((4, 64, 16, 16), _F32, seed + k).relu().to(dtype) for k in range(3)], _t((4, 64, 16, 16), dtype, seed + 3)
+
+
+def _triple_bias_grads(model, opt):
+    """conv name → its bias gradient where the fused step reads it (None: no gradient was made)"""
+    out = {}
+    for name in _TRIPLE:
+        b = getattr(model, name).bias
+        if b is None:
+            continue
+        if getattr(getattr(model, name), "_sod_b16", None) is not None:
+            out[name] = opt.flat.view16(opt.flat.grad16, b).clone()
+        else:
+            out[name] = None if b.grad is None else b.grad.clone()
+    return out
+
+
+def _amp_off():
+    from distributed_sod_project_b200 import amp
+    amp._cfg.update(enabled=False, dynamic=False, scale=1.0, good_steps=0, growth_interval=2000, owner=None, dev=None)
+
+
+@pytest.mark.parametrize("variant", ["all", "m2m_frozen", "l2m_frozen", "h2m_nobias", "m2m_nobias", "l2m_nobias"])
+@pytest.mark.parametrize("train", [pytest.param(True, id="train"), pytest.param(False, id="eval")])
+def test_conv3_folded_biases_get_the_same_bits(train, variant):
+    """every trainable bias of the three gets the same bits of Σ dz — the first through the kernel's first slot, the
+    other two through `b2 + b3` in the second (autograd routes that slot's gradient on) — whether the .grad is bound
+    fp32, bound 16-bit or a temporary, with `b2` or `b3` frozen or one convolution without a bias (so the second slot is
+    a leaf); a frozen bias gets nothing.  The fp32 bound and temporary paths give the same bits.  In eval mode Σ dz is
+    not zero in exact arithmetic: it must be within rounding of Σ dy·[y > 0]·γ/√(running_var + eps) in float64."""
+    got = {}
+    for path in _GRAD_PATHS:
+        model, opt, dtype = _triple(path, variant)
+        try:
+            model.train(train)
+            if opt is not None:
+                _clear_grads(opt)
+            (h, m, l), dy = _triple_inputs(dtype, 41)  # noqa: E741
+            y = model(h, m, l)
+            y.backward(dy)
+            grads = _triple_bias_grads(model, opt)
+        finally:
+            _amp_off()
+        trainable = [n for n in _TRIPLE if getattr(model, n).bias is not None and getattr(model, n).bias.requires_grad]
+        assert len(trainable) == (3 if variant == "all" else 2)
+        for n in set(grads) - set(trainable):                       # frozen: its buffer untouched, or no .grad at all
+            assert grads[n] is None or float(grads[n].abs().max()) == 0.0, (path, n)
+        first = grads[trainable[0]]
+        assert first.dtype == dtype and float(first.abs().max()) > 0, path
+        for n in trainable[1:]:
+            assert torch.equal(grads[n], first), f"{path} {variant}: {n} differs from {trainable[0]}"
+        if not train:
+            bn = model.bnm
+            scale = bn.weight.detach().double() / torch.sqrt(bn.running_var.double() + bn.eps)
+            want = (dy.double() * (y.detach() > 0) * scale.view(1, -1, 1, 1)).sum(dim=(0, 2, 3))
+            _close(first, want, 1e-4 if dtype == _F32 else 2e-2, f"{path} eval Σ dz")
+        got[path] = first
+    assert torch.equal(got["bound32"], got["temporary"])
+
+
+@pytest.mark.parametrize("path", _GRAD_PATHS)
+def test_conv3_second_backward_doubles_the_bias_gradients(path):
+    """a second backward without zeroing doubles every bias gradient: exactly where autograd adds g + g (fp32, and the
+    16-bit .grad of `b2` / `b3`, which autograd accumulates from the second slot's temporary), within one rounding of
+    the 16-bit type where the kernel adds its fp32 Σ dz into the bound 16-bit .grad of `b1`"""
+    model, opt, dtype = _triple(path)
+    try:
+        if opt is not None:
+            _clear_grads(opt)
+        (h, m, l), dy = _triple_inputs(dtype, 45)  # noqa: E741
+        runs = []
+        for _ in range(2):
+            model(h, m, l).backward(dy)
+            runs.append(_triple_bias_grads(model, opt))
+    finally:
+        _amp_off()
+    first, second = runs
+    assert all(torch.equal(first[n], first["h2m"]) for n in _TRIPLE)
+    for n in _TRIPLE:
+        if dtype == _F32 or n != "h2m":
+            assert torch.equal(second[n], 2 * first[n]), (path, n)
+        else:
+            g1, g2 = first[n].float(), second[n].float()
+            assert bool(((g2 - 2 * g1).abs() <= torch.finfo(dtype).eps * (2 * g1).abs() + torch.finfo(dtype).tiny).all())
+
+
+@pytest.mark.parametrize("dtype", [pytest.param(_F32, id="fp32"), pytest.param(_BF16, id="bf16")])
+def test_zero_grad_clears_a_backward_through_the_non_leaf_bias_slot(dtype):
+    """γ/β and `b1` frozen (and, in fp32, the weights): the only gradient writes of the backward are `b2`'s and `b3`'s,
+    which autograd accumulates from conv3_bn_act's second slot.  After a step, such a backward and zero_grad, the next
+    backward must see a clean buffer."""
+    model, opt, _ = _triple("bound16" if dtype == _BF16 else "bound32", "h2m_frozen", frozen_affine=True)
+    try:
+        if dtype == _F32:
+            for n in _TRIPLE:
+                getattr(model, n).weight.requires_grad_(False)
+        (h, m, l), dy = _triple_inputs(dtype, 47)  # noqa: E741
+        opt.zero_grad()
+        model(h, m, l).backward(dy)
+        once = _triple_bias_grads(model, opt)
+        assert float(once["m2m"].abs().max()) > 0 and torch.equal(once["m2m"], once["l2m"])
+        opt.step()
+        model(h, m, l).backward(dy)                     # after the step: writes only the non-leaf slot makes
+        opt.zero_grad()
+        model(h, m, l).backward(dy)
+        again = _triple_bias_grads(model, opt)
+        for n in ("m2m", "l2m"):
+            assert torch.equal(again[n], once[n]), f"stale {n} bias gradient survived zero_grad"
+    finally:
+        _amp_off()
+
+
+@pytest.mark.parametrize("shadowed", [pytest.param(("h2m",), id="b1_16bit"), pytest.param(("m2m", "l2m"), id="b23_16bit"),
+                                      pytest.param(("h2m", "m2m"), id="b1_b2_16bit")])
+def test_conv3_biases_of_mixed_dtypes_are_refused(shadowed):
+    """the SyncBN kernel reads both folded-bias slots under one dtype code, so a conv3_bn_act call whose slots would hold
+    biases of different dtypes raises SodError before any launch.  (`b2 + b3` of two dtypes is promoted by the add, so
+    what counts is the two slots.)  amp does not produce the case: `test_amp_gives_every_neck_bias_one_dtype`."""
+    from distributed_sod_project_b200 import _lib
+    from distributed_sod_project_b200.syncbn import convert_syncbn_model
+    torch.manual_seed(42)
+    model = convert_syncbn_model(_Triple().cuda().to(memory_format=torch.channels_last))
+    for n in shadowed:                              # a 16-bit shadow on some of the three only, as amp never leaves it
+        conv = getattr(model, n)
+        conv._sod_w16 = conv.weight.detach().to(_BF16).requires_grad_()
+        conv._sod_b16 = conv.bias.detach().to(_BF16).requires_grad_()
+    (h, m, l), _ = _triple_inputs(_BF16, 49)  # noqa: E741
+    launches = _lib.launches
+    with torch.autocast("cuda", dtype=_BF16), pytest.raises(_lib.SodError, match="share a dtype"):
+        model(h, m, l)
+    assert _lib.launches == launches
+
+
+def test_amp_gives_every_neck_bias_one_dtype(engines):
+    """under amp every biased convolution of the LightAIM neck has a 16-bit shadow bias of the activation dtype, so no
+    conv_bn_act / conv3_bn_act call of the neck hands the SyncBN kernel biases of two dtypes"""
+    for dtype in (_BF16, _F16):
+        tr = engines("aim_res50", dtype)
+        convs = [m for m in tr.module.trans.modules() if isinstance(m, nn.Conv2d)]
+        assert convs and all(c.bias is not None for c in convs)
+        assert all(getattr(c, "_sod_b16", None) is not None and c._sod_b16.dtype == dtype for c in convs)
 
 
 # ---- seam cases on one GroupNorm32 and the weight-standardised convolutions -------------------------------------------

@@ -1,13 +1,17 @@
-"""The resampling kernels of csrc/resample.cu and csrc/maxpool.cu in every launch regime of this GPU, element by element
-against float64 (oracle/resample.py), and `sod_colsum` bit for bit against an fp32 replay of its summation order.
+"""The resampling kernels of csrc/resample.cu, csrc/maxpool.cu and csrc/nearest.cu in every launch regime of this GPU,
+element by element against float64 (oracle/resample.py), the nearest ×2 kernels bit for bit (the forward against torch,
+the backward against the fixed-order restatement of tests/_nearest.py), and `sod_colsum` bit for bit against an fp32
+replay of its summation order.
 
 Which threads make a second pass, which stay idle and which run the colsum tail is decided at launch time from the SM
-count.  oracle/resample_geometry.py picks, for the device the test runs on, the smallest shape that puts each of the six
-grid-stride kernels (bilinear ×2, 2×2 average pool, 3×3/2 max pool; forward and backward) in each wave regime (a partial
-wave below the 16·#SMs cap, one full pass, a full pass plus a ragged one, two or more passes ragged and exact), and the
-row counts that give `sod_colsum` every L = C/8 from 1 to 256, a grid below and at its cap, every tail residue q mod 4,
-idle threads and a single row.  The shapes res50 passes to each kernel at 256², 320² and 384² (bs 16) are recorded by
-wrapping the library calls of one training iteration, and are run too.  Each kernel runs on its own: the backward
+count.  oracle/resample_geometry.py picks, for the device the test runs on, the smallest shape that puts each of the
+eight grid-stride kernels (bilinear ×2, 2×2 average pool, 3×3/2 max pool, nearest ×2; forward and backward) in each wave
+regime (a partial wave below the 16·#SMs cap, one full pass, a full pass plus a ragged one, two or more passes ragged
+and exact), and the row counts that give `sod_colsum` every L = C/8 from 1 to 256, a grid below and at its cap, every
+tail residue q mod 4, idle threads and a single row.  The shapes res50 passes to each kernel at 256², 320² and 384²
+(bs 16), and the twelve nearest up-sample shapes of aim_res50 at 320² and 352² (bs 16; at 320² the 64-channel 80² maps
+are 819 200 packets, more than one pass of a 132-SM H100's 540 672 threads), are recorded by wrapping the library calls
+of one training iteration, and are run too.  Each kernel runs on its own: the backward
 kernels get their dy (and the max-pool's window positions) from the test, not from the forward kernel.
 
 Inputs come in three tiers.
@@ -27,7 +31,7 @@ Inputs come in three tiers.
   subnormals, which must not be flushed.  Where the oracle's result in the dtype is not finite the kernel must give
   the same (NaN where NaN, the same infinity); elsewhere the random-tier bound holds.  The average pool sums its four
   inputs in fp32 before the quarter, as torch's kernel does, so its windows keep that sum finite (M only in fp16, where
-  4M fits fp32).
+  4M fits fp32).  The nearest kernels are compared by bits in every tier, NaN by class (its payload is the device's).
 
 Refusals: null pointers, 2-byte misalignment, n/h/w ≤ 0, C % 8, colsum C = 24 and 4096, a short workspace and an
 unknown dtype code each return their code and leave a sentinel-filled output untouched.
@@ -37,6 +41,9 @@ import zlib
 
 import pytest
 import torch
+import torch.nn.functional as F
+
+from _nearest import upsample2x_nearest_bwd
 
 from oracle import resample as ors
 from oracle import resample_geometry as geo
@@ -126,6 +133,21 @@ def max_bwd(dy, arg, h, w):
     n, c = dy.shape[:2]
     dx = _cl((n, c, h, w), dy.dtype)
     _run("sod_maxpool3x3s2_bwd", dy.data_ptr(), arg.data_ptr(), dx.data_ptr(), n, h, w, c, _lib().dtype_code(dy.dtype),
+         _lib().stream_ptr())
+    return dx
+
+
+def near_fwd(x):
+    n, c, h, w = x.shape
+    y = _cl((n, c, 2 * h, 2 * w), x.dtype)
+    _run("sod_upsample2x_nearest_fwd", x.data_ptr(), y.data_ptr(), n, h, w, c, _lib().dtype_code(x.dtype), _lib().stream_ptr())
+    return y
+
+
+def near_bwd(dy):
+    n, c, h2, w2 = dy.shape
+    dx = _cl((n, c, h2 // 2, w2 // 2), dy.dtype)
+    _run("sod_upsample2x_nearest_bwd", dy.data_ptr(), dx.data_ptr(), n, h2 // 2, w2 // 2, c, _lib().dtype_code(dy.dtype),
          _lib().stream_ptr())
     return dx
 
@@ -222,6 +244,19 @@ def assert_matches(got, ref, tol, dtype, what):
                              f"float64 {float(ref[tuple(i)])!r}" + ("" if tol is None else f", bound {float(tol[tuple(i)]):.3g}"))
 
 
+def assert_same_bits(got, want, what):
+    """bit for bit, NaN by class (a NaN's payload is the device's)"""
+    bits = {4: torch.int32, 2: torch.int16}[got.element_size()]
+    g, w = got.contiguous(), want.contiguous()
+    nan = w.isnan()
+    assert torch.equal(g.isnan(), nan), f"{what}: NaN at other positions ({int((g.isnan() != nan).sum())})"
+    bad = (g.view(bits) != w.view(bits)) & ~nan
+    if bool(bad.any()):
+        i = bad.nonzero()[0].tolist()
+        raise AssertionError(f"{what}: {int(bad.sum())} of {bad.numel()} elements differ, first at {i}: got "
+                             f"{float(g[tuple(i)])!r}, want {float(w[tuple(i)])!r}")
+
+
 def _fp32_floor(dtype, ops):
     """the absolute rounding of `ops` fp32 operations on subnormal fp32 values"""
     return ops * 2.0 ** -149 if dtype == torch.float32 else 0.0
@@ -279,12 +314,18 @@ def check_kernel(kernel, shape, dtype, tier, seed):
         tol = None if exact else (ulp(ref, dtype) + 2.0 ** -22 * ors.maxpool_bwd(d64.abs(), aref, h, w).permute(0, 3, 1, 2)
                                   .nan_to_num(posinf=0.0) + _fp32_floor(dtype, 4))
         assert_matches(dx, ref, tol, dtype, f"{kernel} {tier}")
+    elif kernel == "nearest_fwd":
+        x = make(shape, dtype, tier, seed)
+        assert_same_bits(near_fwd(x), F.interpolate(x, scale_factor=2, mode="nearest"), f"{kernel} {tier}")
+    elif kernel == "nearest_bwd":
+        dy = make((n, c, 2 * h, 2 * w), dtype, tier, seed, "dy")
+        assert_same_bits(near_bwd(dy), upsample2x_nearest_bwd(dy), f"{kernel} {tier}")
     else:
         raise KeyError(kernel)
 
 
-# ---- the six grid-stride kernels in every wave regime ------------------------------------------------------------------
-WAVE_CASES = [(k, d, wv) for k in geo.KERNELS for d in geo.DTYPES for wv in geo.WAVES]
+# ---- the eight grid-stride kernels in every wave regime ----------------------------------------------------------------
+WAVE_CASES = [(k, d, wv) for k in geo.GRID_STRIDE_KERNELS for d in geo.DTYPES for wv in geo.WAVES]
 
 
 @pytest.mark.parametrize("kernel, dtype, wave", WAVE_CASES, ids=[f"{k}-{d}-{w}" for k, d, w in WAVE_CASES])
@@ -302,7 +343,7 @@ SMALL = [(1, 8, 1, 1), (3, 8, 1, 5), (2, 16, 7, 1), (2, 32, 5, 7), (1, 128, 2, 9
 
 
 @pytest.mark.parametrize("dtype", geo.DTYPES)
-@pytest.mark.parametrize("kernel", geo.KERNELS)
+@pytest.mark.parametrize("kernel", geo.GRID_STRIDE_KERNELS)
 def test_small_and_degenerate_shapes(kernel, dtype):
     for i, (n, c, h, w) in enumerate(SMALL):
         shape = (n, c, 2 * h, 2 * w) if kernel.startswith("avgpool") else (n, c, h, w)
@@ -327,14 +368,15 @@ def test_upsample_border_infinities_stay_infinite():
         assert_matches(y, want, None, dtype, "border")
 
 
-# ---- the shapes res50 passes to each kernel -----------------------------------------------------------------------------
+# ---- the shapes res50 and aim_res50 pass to each kernel ----------------------------------------------------------------
 _RES50: dict = {}
 
 
-def _res50_shapes(size):
-    """{kernel: sorted forward-input shapes} of one bs-16 res50 training iteration at size², recorded at the C ABI"""
-    if size in _RES50:
-        return _RES50[size]
+def _res50_shapes(size, model="res50"):
+    """{kernel: sorted forward-input shapes} of one bs-16 `model` training iteration at size², recorded at the C ABI;
+    "nearest_calls": the number of nearest forward launches"""
+    if (model, size) in _RES50:
+        return _RES50[(model, size)]
     from distributed_sod_project_b200 import resample
     from distributed_sod_project_b200.engine import Trainer
     from distributed_sod_project_b200.synthetic import synth_batch
@@ -360,7 +402,7 @@ def _res50_shapes(size):
         def lib(self):
             return _Lib(real.lib())
 
-    tr = Trainer(model_name="res50", dtype=torch.bfloat16, channels_last=True, use_graph=False)
+    tr = Trainer(model_name=model, dtype=torch.bfloat16, channels_last=True, use_graph=False)
     x, m = synth_batch(7, 16, size)
     resample._lib = _Rec()
     try:
@@ -383,16 +425,21 @@ def _res50_shapes(size):
             k, s = "maxpool_bwd", (a[3], a[6], a[4], a[5])
         elif name == "sod_colsum":
             k, s = "colsum", (a[2], a[3])
+        elif name in ("sod_upsample2x_nearest_fwd", "sod_upsample2x_nearest_bwd"):
+            k, s = ("nearest_fwd" if name.endswith("fwd") else "nearest_bwd"), (a[2], a[5], a[3], a[4])
         else:
             continue
         shapes.setdefault(k, set()).add(s)
-    _RES50[size] = {k: sorted(v) for k, v in shapes.items()}
-    return _RES50[size]
+    out = {k: sorted(v) for k, v in shapes.items()}
+    out["nearest_calls"] = sum(name == "sod_upsample2x_nearest_fwd" for name, _ in calls)
+    _RES50[(model, size)] = out
+    return out
 
 
 @pytest.mark.parametrize("size", [256, 320, 384])
 def test_res50_shapes(size):
-    shapes = _res50_shapes(size)
+    shapes = dict(_res50_shapes(size))
+    assert shapes.pop("nearest_calls") == 0                                  # res50 has no nearest up-sample
     assert set(shapes) == set(geo.KERNELS) | {"colsum"}, sorted(shapes)
     for kernel in geo.KERNELS:
         for i, shape in enumerate(shapes[kernel]):
@@ -403,6 +450,22 @@ def test_res50_shapes(size):
         for dtype in geo.DTYPES:
             for tier in ("exact", "random"):
                 check_colsum(rows, c, TORCH_DT[dtype], tier, seed=rows + c)
+
+
+@pytest.mark.parametrize("size", [320, 352])
+def test_aim_res50_nearest_shapes(size):
+    """the twelve nearest up-samples of one bs-16 aim_res50 iteration (64 channels at S/4 … S/32, 1024 at S/32), forward
+    and backward, in every dtype and tier; at 320² the largest run the grid-stride loop twice on a 132-SM H100"""
+    shapes = _res50_shapes(size, "aim_res50")
+    assert shapes["nearest_calls"] == 12
+    q = size // 4
+    want = sorted({(16, 64, q >> k, q >> k) for k in range(4)} | {(16, 1024, q // 8, q // 8)})
+    assert shapes["nearest_fwd"] == shapes["nearest_bwd"] == want, shapes["nearest_fwd"]
+    for kernel in ("nearest_fwd", "nearest_bwd"):
+        for i, shape in enumerate(shapes[kernel]):
+            for dtype in geo.DTYPES:
+                for j, tier in enumerate(TIERS):
+                    check_kernel(kernel, shape, TORCH_DT[dtype], tier, seed=size + 10 * i + j)
 
 
 # ---- sod_colsum ----------------------------------------------------------------------------------------------------------
@@ -476,7 +539,7 @@ def _refuse(fn, args, code, outs, what):
         assert bool((o == SENTINEL).all()), f"{what}: the output was written"
 
 
-@pytest.mark.parametrize("entry", ["up_fwd", "up_bwd", "avg_fwd", "avg_bwd", "max_fwd", "max_bwd"])
+@pytest.mark.parametrize("entry", ["up_fwd", "up_bwd", "avg_fwd", "avg_bwd", "max_fwd", "max_bwd", "near_fwd", "near_bwd"])
 def test_grid_stride_entries_refuse_bad_arguments(entry):
     L = _lib()
     lib, st, f32 = L.lib(), L.stream_ptr(), L.SOD_F32
@@ -505,7 +568,8 @@ def test_grid_stride_entries_refuse_bad_arguments(entry):
         ptrs, optional = [0, 1, 2], []
     else:
         fn = {"up_bwd": lib.sod_upsample2x_bilinear_bwd, "avg_fwd": lib.sod_avgpool2x2_fwd,
-              "avg_bwd": lib.sod_avgpool2x2_bwd}[entry]
+              "avg_bwd": lib.sod_avgpool2x2_bwd, "near_fwd": lib.sod_upsample2x_nearest_fwd,
+              "near_bwd": lib.sod_upsample2x_nearest_bwd}[entry]
 
         def call(p=(s, o), dims=(n, h, w, c), dt=f32):
             return (*p, *dims, dt, st)

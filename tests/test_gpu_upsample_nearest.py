@@ -1,7 +1,8 @@
 """The nearest ×2 kernels of csrc/nearest.cu (`sod_upsample2x_nearest_fwd` / `_bwd`, LightAIM's up-sampling) on the
 GPU: the forward bit for bit against torch, the backward bit for bit against the fixed-order restatement of
-tests/_nearest.py and, in 16 bit, within one rounding of the float64 sum; reruns and CUDA-graph replay bit-identical;
-every refusal code."""
+tests/_nearest.py and, in 16 bit, within one rounding of the float64 sum; infinities, NaN, −0 and sums past the largest
+finite value through the backward; reruns and CUDA-graph replay bit-identical; every refusal code.  Every launch regime
+of both kernels is in tests/test_gpu_resample_regimes.py."""
 from __future__ import annotations
 
 import pytest
@@ -62,6 +63,57 @@ def test_nearest_matches_torch_and_the_fixed_order_oracle(shape, dtype):
         exact = upsample2x_nearest_bwd64(dy)
         ulp = torch.finfo(dtype).eps * exact.abs().clamp_min(torch.finfo(dtype).tiny)
         assert bool(((dx.double() - exact).abs() <= ulp).all())
+
+
+def _classes(t):
+    """per element: 0 finite, 1 NaN, 2 +inf, 3 −inf"""
+    return t.isnan().int() + 2 * t.isposinf().int() + 3 * t.isneginf().int()
+
+
+@pytest.mark.parametrize("dtype", DTYPES, ids=str)
+def test_backward_special_values(dtype):
+    """±inf, NaN and −0 in dy; four taps of the largest finite value M (their sum overflows the dtype: in fp32 for fp32
+    and bf16, in the final rounding for fp16, where 4M fits fp32), four of M/4 (exactly M), ±M alternating (exactly 0);
+    in fp16 four taps summing to 65536 (past 65504: inf) and to 65512 (below the 65520 midpoint: 65504).  The backward
+    equals the fixed-order oracle bit for bit (NaN by class) and torch's own nearest backward class for class (NaN,
+    +inf, −inf, finite)."""
+    n, c, h, w = 2, 16, 5, 6
+    big = torch.finfo(dtype).max
+    inf, nan = float("inf"), float("nan")
+    dy = _x((n, c, 2 * h, 2 * w), torch.float32, 21)
+    dy[0, 0, 0, 0] = inf                                   # one +inf tap, first window
+    dy[0, 1, 0, 0], dy[0, 1, 1, 1] = inf, -inf             # +inf + −inf: NaN
+    dy[0, 2, 2, 3] = nan
+    dy[n - 1, 3, 2 * h - 1, 2 * w - 1] = -inf              # last window, last channel-group row
+    dy[:, 4] = -0.0                                        # (((0 + −0) + −0) + −0) + −0 = +0
+    dy[:, 5], dy[:, 5, 0::2, :] = 0.0, -0.0                 # −0 and +0 taps
+    dy[:, 6] = big
+    dy[:, 7] = big / 4
+    dy[:, 8, :, 0::2], dy[:, 8, :, 1::2] = big, -big       # ((0 + M) − M) + M) − M, never past M
+    if dtype == torch.float16:
+        dy[:, 9] = 16384.0
+        dy[:, 10] = 16376.0
+        dy[:, 10, 1::2, 1::2] = 16384.0
+    dy = dy.to(dtype).contiguous(memory_format=torch.channels_last)
+    assert bool(dy[:, 4].signbit().all())
+    x = torch.zeros((n, c, h, w), dtype=dtype, device="cuda").contiguous(memory_format=torch.channels_last)
+    _, dx = _fwd_bwd(x, dy)
+    oracle = upsample2x_nearest_bwd(dy.cpu()).cuda()
+    bits = torch.int32 if dtype == torch.float32 else torch.int16
+    got, want = dx.contiguous(), oracle.contiguous()
+    nan_at = want.isnan()
+    assert torch.equal(got.isnan(), nan_at)
+    assert torch.equal(got.view(bits)[~nan_at], want.view(bits)[~nan_at])
+    # the cases land where they should: NaN, ±inf, +0 and M
+    assert bool(got[0, 1, 0, 0].isnan()) and bool(got[0, 2, 1, 1].isnan())
+    assert float(got[0, 0, 0, 0]) == inf and float(got[n - 1, 3, h - 1, w - 1]) == -inf
+    assert bool((got[:, 4:6] == 0).all()) and not bool(got[:, 4].signbit().any())
+    assert bool(got[:, 6].isposinf().all()) and bool((got[:, 7] == big).all()) and bool((got[:, 8] == 0).all())
+    if dtype == torch.float16:
+        assert bool(got[:, 9].isposinf().all()) and bool((got[:, 10] == 65504.0).all())
+    xr = x.detach().requires_grad_(True)
+    (ref,) = torch.autograd.grad(F.interpolate(xr, scale_factor=2, mode="nearest"), xr, dy)
+    assert torch.equal(_classes(got), _classes(ref))
 
 
 @pytest.mark.parametrize("dtype", DTYPES, ids=str)

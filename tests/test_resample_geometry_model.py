@@ -2,7 +2,7 @@
 on the CPU.
 
 The GPU regime tests (test_gpu_resample_regimes.py) pick their shapes with this model for the device they run on.
-Here: the model's constants are the ones in csrc/resample.cu and csrc/maxpool.cu; the grid-stride loops and the colsum
+Here: the model's constants are the ones in csrc/resample.cu, csrc/maxpool.cu and csrc/nearest.cu; the grid-stride loops and the colsum
 row loop visit every packet / row exactly once; every regime cell is reachable on a 132-SM H100 SXM and a 114-SM H100
 PCIe; and the replay of the colsum order equals an exact sum on integer data.
 """
@@ -25,7 +25,7 @@ def _src(name):
 
 
 def test_constants_match_the_kernel_sources():
-    for name in ("resample.cu", "maxpool.cu"):
+    for name in ("resample.cu", "maxpool.cu", "nearest.cu"):
         src = _src(name)
         assert int(re.search(r"constexpr int kThreads = (\d+);", src).group(1)) == geo.K_THREADS
         body = re.search(r"static unsigned grid_for\(long long packets\) \{(.*?)\n\}", src, re.S).group(1)
@@ -50,6 +50,10 @@ def test_constants_match_the_kernel_sources():
     assert "packets = static_cast<long long>(n) * 2 * h * 2 * w * (c / 8);" in src
     assert "packets = static_cast<long long>(n) * 2 * h_out * 2 * w_out * (c / 8);" in src
     assert "packets = static_cast<long long>(n) * ho * wo * (c / 8);" in _src("maxpool.cu")
+    # the nearest kernels: one thread per input packet, forward and backward
+    src = _src("nearest.cu")
+    assert src.count("const long long packets = static_cast<long long>(n) * h * w * (c / 8);") == 2
+    assert src.count("<<<grid_for(packets), kThreads, 0, s>>>") == 2
 
 
 @pytest.mark.parametrize("sm_count", [1, 3, 132])
@@ -68,7 +72,7 @@ def test_grid_stride_loops_visit_every_packet_once(sm_count):
 
 @pytest.mark.parametrize("sm_count", SM_COUNTS)
 def test_every_wave_cell_is_reachable(sm_count):
-    for kernel in geo.KERNELS:
+    for kernel in geo.GRID_STRIDE_KERNELS:
         for wave in geo.WAVES:
             shape = geo.select(kernel, wave, sm_count)
             p = geo.packets(kernel, shape)
